@@ -117,6 +117,35 @@ typedef struct {
 int t2v_bgemm(const T2VMat* A, const T2VMat* B, void* C, int64_t ldc, int64_t c_stride_z1, int64_t c_stride_z2,
               int32_t M, int32_t N, int32_t K, int32_t Z1, int32_t Z2, float alpha, int32_t out_mode, void* stream);
 
+/* The GEMM launches the four entry points above would make for a problem on a device with `sm_count` SMs, computed on the
+ * host without touching a device: the tiling, split-K, pipeline and epilogue decisions of the planner, one record per
+ * launch (t2v_conv_dgrad with stride 2 makes one launch per output parity class).  The planner overrides T2V_FORCE_BN,
+ * T2V_FORCE_SPLITS, T2V_FORCE_FWD_SPLITS, T2V_FORCE_STAGES, T2V_NO_SPLIT and T2V_NO_ROWSUM_FUSE are read from the environment
+ * on every call, as the entry points do.  Pointers are assumed 16-byte aligned.  Writes min(result, max_out) records and
+ * returns the number of launches, or a negative error for a problem the entry point would reject.                   */
+enum { T2V_GEMM_CONV_FWD = 0, T2V_GEMM_CONV_DGRAD = 1, T2V_GEMM_CONV_WGRAD = 2, T2V_GEMM_BGEMM = 3 };
+enum { T2V_FOLLOW_NONE = 0, T2V_FOLLOW_SPLITK_FINISH = 1, T2V_FOLLOW_CHANNEL_STATS = 2, T2V_FOLLOW_COLSUM = 3 };
+typedef struct {
+    int32_t kind;          /* T2V_GEMM_*                                                                           */
+    int32_t N, H, W, Cin, Cout, KH, KW, stride, pad_h0, pad_h1, pad_w0, pad_w1;   /* convolutions, as in t2v_conv_*   */
+    int32_t workspace;     /* fwd / dgrad: the caller passes split-K scratch (T2VEpilogue.workspace != NULL)          */
+    int32_t stats_rows;    /* fwd: GroupNorm statistics requested, T2VEpilogue.stats_rows (0: not requested)          */
+    int32_t dbias;         /* wgrad: t2v_conv_wgrad_bias rather than t2v_conv_wgrad                                 */
+    int32_t gemm_m, gemm_n, gemm_k, z1, z2, b_kmajor, out_mode;   /* bgemm: M, N, K, Z1, Z2, B->kmajor, out_mode      */
+} T2VGemmProblem;
+typedef struct {
+    int32_t block_n, num_stages;   /* wgmma N, pipeline stages                                                       */
+    int32_t splits, kb_per_split;  /* split-K factor (1: none) and k-blocks per split (0 when not split)              */
+    int32_t ksplit_var;            /* tile variable that selects the k-range (-1: none)                              */
+    int32_t num_tiles, grid;       /* work tiles, persistent CTAs = min(num_tiles, sm_count)                         */
+    int32_t box[3];                /* pixel box (w, h, n) of a tile's 128 rows                                       */
+    int32_t tdim[6], kdim[3];      /* tile grid (t[0] = N tiles) and k-block grid                                    */
+    int32_t flags;                 /* epilogue work chosen by the planner: 16 GroupNorm statistics, 32 bias gradient */
+    int32_t st[5];                 /* statistics row -> sample map (cw, ch, cn, div, seg) when flags has 16          */
+    int32_t follow;                /* T2V_FOLLOW_*: the pass that completes this launch                               */
+} T2VGemmPlan;
+int t2v_gemm_plan(const T2VGemmProblem* problem, int32_t sm_count, T2VGemmPlan* out, int32_t max_out);
+
 /* Fused attention (head_dim 64): O = softmax(Q K^T / 8) V per (batch, head) without materialising the score matrix,
  * plus its backward; replaces the t2v_bgemm / t2v_softmax composition for Transformer2DModel's self- and cross-attention
  * (diffusers AttnProcessor2_0 -> F.scaled_dot_product_attention in the reference, train.py:138-152).

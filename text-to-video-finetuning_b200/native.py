@@ -61,8 +61,20 @@ class Mat(ctypes.Structure):
                 ("stride_z2", ctypes.c_int64), ("kmajor", ctypes.c_int32)]
 
 
+class GemmProblem(ctypes.Structure):
+    _fields_ = [(f, ctypes.c_int32) for f in (
+        "kind", "N", "H", "W", "Cin", "Cout", "KH", "KW", "stride", "pad_h0", "pad_h1", "pad_w0", "pad_w1",
+        "workspace", "stats_rows", "dbias", "gemm_m", "gemm_n", "gemm_k", "z1", "z2", "b_kmajor", "out_mode")]
+
+
+class GemmPlan(ctypes.Structure):
+    _fields_ = [(f, ctypes.c_int32) for f in ("block_n", "num_stages", "splits", "kb_per_split", "ksplit_var", "num_tiles", "grid")] + [
+        ("box", ctypes.c_int32 * 3), ("tdim", ctypes.c_int32 * 6), ("kdim", ctypes.c_int32 * 3), ("flags", ctypes.c_int32),
+        ("st", ctypes.c_int32 * 5), ("follow", ctypes.c_int32)]
+
+
 EXPORTS = [
-    "t2v_version", "t2v_last_error", "t2v_launch_count", "t2v_stream_capture_id", "t2v_channel_stats", "t2v_conv_fwd", "t2v_conv_dgrad", "t2v_conv_workspace_bytes", "t2v_conv_wgrad", "t2v_conv_wgrad_bias", "t2v_bgemm", "t2v_flash_attn_fwd", "t2v_flash_attn_bwd_splits", "t2v_flash_attn_bwd",
+    "t2v_version", "t2v_last_error", "t2v_launch_count", "t2v_stream_capture_id", "t2v_channel_stats", "t2v_conv_fwd", "t2v_conv_dgrad", "t2v_conv_workspace_bytes", "t2v_conv_wgrad", "t2v_conv_wgrad_bias", "t2v_bgemm", "t2v_gemm_plan", "t2v_flash_attn_fwd", "t2v_flash_attn_bwd_splits", "t2v_flash_attn_bwd",
     "t2v_groupnorm_workspace_bytes", "t2v_groupnorm_fwd", "t2v_groupnorm_bwd", "t2v_layernorm_fwd", "t2v_layernorm_bwd",
     "t2v_latents_to_nhwc8", "t2v_nhwc8_to_latents", "t2v_mse_loss", "t2v_vae_sample", "t2v_geglu_fwd", "t2v_geglu_bwd", "t2v_silu_f32_to_bf16",
     "t2v_silu_bwd_f32", "t2v_silu_bf16", "t2v_silu_bf16_bwd", "t2v_add_bf16", "t2v_add_f32", "t2v_dropout_scale_add", "t2v_scale_bf16", "t2v_cast_f32_bf16", "t2v_embed_tokens", "t2v_gelu_bf16", "t2v_frames_u8_to_nhwc8", "t2v_scale_cast_f32_bf16", "t2v_cast_bf16_f32", "t2v_sqnorm_chunks", "t2v_adamw_prepare", "t2v_adamw_chunks", "t2v_counter_add", "t2v_upsample_nearest_fwd",
@@ -87,6 +99,7 @@ def _declare(lib):
     lib.t2v_conv_workspace_bytes.restype = i64
     lib.t2v_conv_workspace_bytes.argtypes = [i32] * 13
     lib.t2v_bgemm.argtypes = [ctypes.POINTER(Mat), ctypes.POINTER(Mat), vp, i64, i64, i64, i32, i32, i32, i32, i32, f32, i32, vp]
+    lib.t2v_gemm_plan.argtypes = [ctypes.POINTER(GemmProblem), i32, ctypes.POINTER(GemmPlan), i32]
     lib.t2v_flash_attn_fwd.argtypes = [vp] * 5 + [i32] * 5 + [i64] * 8 + [vp]
     lib.t2v_flash_attn_bwd.argtypes = [vp] * 11 + [i32] * 5 + [i64] * 14 + [vp]
     lib.t2v_flash_attn_bwd_splits.restype = i32

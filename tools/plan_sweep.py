@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """Planner sweep for forward / data-gradient GEMMs: for each listed shape, times the planner's own choice and every forced
 (wgmma N, split-K) combination (T2V_FORCE_BN / T2V_FORCE_FWD_SPLITS), L2-cold (rotating
-operand sets), CUDA-graph replay, CUDA events.  The CSV lines are what the cost model in csrc/gemm_plan.cu::choose_tiling is
-fitted to; cuBLAS on the same shape is printed as the yardstick.
+operand sets), CUDA-graph replay, CUDA events.  The CSV lines are what the fwd / dgrad cost model in csrc/gemm_plan.cu
+(fwd_cost) is fitted to; cuBLAS on the same shape is printed as the yardstick.
   python tools/plan_sweep.py > gpurun_out/plan_sweep.txt"""
 import itertools
 import os
