@@ -108,7 +108,7 @@ def test_problems():
         out += [(conv_problem("wgrad", *c), env), (conv_problem("wgrad", *c, dbias=1), env)]
     for c in T.SPLITK_CASES:
         out += [(conv_problem("fwd", *c, workspace=1), {}), (conv_problem("dgrad", *c, workspace=1), {})]
-    for M, N, K, Z1, Z2, _, bk, mode in T.BGEMM_CASES:
+    for M, N, K, Z1, Z2, _, bk, mode, _ in T.BGEMM_CASES:
         out.append((bgemm_problem(M, N, K, Z1, Z2, bk, mode), {}))
     return out
 

@@ -69,14 +69,15 @@ def test_conv_fwd(case):
     torch.cuda.synchronize()
     e = rel_err(y, ref)
     assert e < 1e-2, f"plain conv rel err {e}"
-    # fused epilogue, fp32 output
-    y2 = torch.full((N, Ho, Wo, Co), float("nan"), device="cuda", dtype=torch.float32)
-    epi = nat.Epilogue(bias.data_ptr(), rowbias.data_ptr(), res.data_ptr(), 0.5, 1, 1)
-    nat.check(nat.lib().t2v_conv_fwd(P(x), P(w), P(y2), N, H, W, Ci, Co, KH, KW, s, *pads, ctypes.byref(epi), stream()))
-    torch.cuda.synchronize()
+    # fused epilogue, fp32 and bf16 output
     ref2 = 0.5 * ref + bias + rowbias[:, None, None, :] + res.float()
-    e = rel_err(y2, ref2)
-    assert e < 2e-3, f"epilogue conv rel err {e}"
+    for out_fp32, tol in ((1, 2e-3), (0, 1e-2)):
+        y2 = torch.full((N, Ho, Wo, Co), float("nan"), device="cuda", dtype=torch.float32 if out_fp32 else torch.bfloat16)
+        epi = nat.Epilogue(bias.data_ptr(), rowbias.data_ptr(), res.data_ptr(), 0.5, out_fp32, 1)
+        nat.check(nat.lib().t2v_conv_fwd(P(x), P(w), P(y2), N, H, W, Ci, Co, KH, KW, s, *pads, ctypes.byref(epi), stream()))
+        torch.cuda.synchronize()
+        e = rel_err(y2, ref2)
+        assert e < tol, f"epilogue conv rel err {e} (fp32 output: {out_fp32})"
 
 
 DGRAD_CASES = [c for c in CONV_CASES if c[3] % 8 == 0 and c[4] % 8 == 0]
@@ -203,28 +204,28 @@ def test_conv_splitk_scratch(case):
 
 
 BGEMM_CASES = [
-    # M, N, K, Z1, Z2, a_kmajor, b_kmajor, out_mode
-    (1024, 1024, 64, 2, 5, 1, 1, 1),   # S = Q K^T per (frame, head), fp32
-    (1024, 64, 1024, 2, 5, 1, 0, 0),   # O = P V
-    (1024, 80, 64, 2, 5, 1, 1, 1),     # cross-attention scores (Lk 77 -> 80)
-    (200, 64, 136, 1, 3, 1, 0, 0),     # ragged
-    (320, 320, 2000, 1, 1, 0, 0, 2),   # linear wgrad dW = dY^T X (split-K, accumulate)
-    (1024, 64, 1024, 2, 5, 0, 0, 1),   # dV = P^T dO
-    (256, 512, 512, 3, 1, 1, 1, 0),    # VAE-style d=512
+    # M, N, K, Z1, Z2, a_kmajor, b_kmajor, out_mode, ldc
+    (1024, 1024, 64, 2, 5, 1, 1, 1, 1024),   # S = Q K^T per (frame, head), fp32
+    (1024, 64, 1024, 2, 5, 1, 0, 0, 64),     # O = P V
+    (1024, 80, 64, 2, 5, 1, 1, 1, 80),       # cross-attention scores (Lk 77 -> 80)
+    (200, 64, 136, 1, 3, 1, 0, 0, 64),       # ragged
+    (320, 320, 2000, 1, 1, 0, 0, 2, 320),    # linear wgrad dW = dY^T X (split-K, accumulate)
+    (1024, 64, 1024, 2, 5, 0, 0, 1, 64),     # dV = P^T dO
+    (256, 512, 512, 3, 1, 1, 1, 0, 512),     # VAE-style d=512
+    (1024, 77, 64, 2, 5, 1, 1, 1, 77),       # unpadded Lk 77: rows not 16-byte aligned, the epilogue's scalar path
 ]
 
 
 @pytest.mark.parametrize("case", BGEMM_CASES)
 def test_bgemm(case):
     nat = _lib()
-    M, N, K, Z1, Z2, ak, bk, mode = case
+    M, N, K, Z1, Z2, ak, bk, mode, ldc = case
     g = torch.Generator(device="cuda").manual_seed(3)
     A = torch.randn((Z1, Z2, M, K) if ak else (Z1, Z2, K, M), device="cuda", generator=g).bfloat16()
     B = torch.randn((Z1, Z2, N, K) if bk else (Z1, Z2, K, N), device="cuda", generator=g).bfloat16()
     Af = A.float() if ak else A.float().transpose(-1, -2)
     Bf = B.float() if bk else B.float().transpose(-1, -2)
     ref = 0.125 * Af @ Bf.transpose(-1, -2)
-    ldc = (N + 7) // 8 * 8
     dt = torch.bfloat16 if mode == 0 else torch.float32
     C = torch.zeros(Z1, Z2, M, ldc, device="cuda", dtype=dt)
     if mode == 2:

@@ -390,15 +390,16 @@ int plan(const T2VGemmProblem& q, int sms, const Overrides& ov, Launch* l) {
     return planners[q.kind](q, sms, ov, l);
 }
 
-// Finishing pass of a split-K problem that also produces the GroupNorm statistics of its output: a block owns RPB
-// consecutive rows of ONE statistics sample and 256 column quads; a thread loads its quad of all RPB rows up front (independent
-// loads: one memory round trip), finishes them, and adds the column sums with two red.add.v4.
+// Finishing pass of a split-K problem: out = alpha * acc + bias + rowbias + residual and, when `stats` is set, the GroupNorm
+// statistics of out.  A block owns RPB consecutive rows (with statistics: of ONE sample) and 256 column quads; a thread loads
+// its quad of all RPB rows up front (independent loads: one memory round trip), finishes them, and adds the column sums with
+// two red.add.v4.
 template <int RPB>
-__global__ void __launch_bounds__(256) splitk_finish_stats_kernel(const float* __restrict__ acc, const float* __restrict__ bias,
-                                                                  const float* __restrict__ rowbias, const __nv_bfloat16* __restrict__ residual,
-                                                                  void* __restrict__ out, int64_t rows, int C, int64_t rows_per_sample, int rb_div,
-                                                                  int64_t rb_ld, float alpha, int out_fp32, float* __restrict__ stats,
-                                                                  int64_t st_ld, int st_rows) {
+__global__ void __launch_bounds__(256) splitk_finish_kernel(const float* __restrict__ acc, const float* __restrict__ bias,
+                                                            const float* __restrict__ rowbias, const __nv_bfloat16* __restrict__ residual,
+                                                            void* __restrict__ out, int64_t rows, int C, int64_t rows_per_sample, int rb_div,
+                                                            int64_t rb_ld, float alpha, int out_fp32, float* __restrict__ stats,
+                                                            int64_t st_ld, int st_rows) {
     pdl_sync();
     const int64_t r0 = int64_t(blockIdx.x) * RPB;
     const int c = (blockIdx.y * blockDim.x + threadIdx.x) * 4;
@@ -421,7 +422,10 @@ __global__ void __launch_bounds__(256) splitk_finish_stats_kernel(const float* _
         const int64_t r = r0 + i;
         if (r >= rows) break;
         float4 y = v[i];
-        y.x = y.x * alpha + b4.x; y.y = y.y * alpha + b4.y; y.z = y.z * alpha + b4.z; y.w = y.w * alpha + b4.w;
+        y.x *= alpha; y.y *= alpha; y.z *= alpha; y.w *= alpha;
+        if (bias) {
+            y.x += b4.x; y.y += b4.y; y.z += b4.z; y.w += b4.w;
+        }
         if (rowbias) {
             const float4 b = __ldg(reinterpret_cast<const float4*>(rowbias + (r / rows_per_sample / rb_div) * rb_ld + c));
             y.x += b.x; y.y += b.y; y.z += b.z; y.w += b.w;
@@ -442,42 +446,10 @@ __global__ void __launch_bounds__(256) splitk_finish_stats_kernel(const float* _
         s[0] += y.x; s[1] += y.y; s[2] += y.z; s[3] += y.w;
         q[0] += y.x * y.x; q[1] += y.y * y.y; q[2] += y.z * y.z; q[3] += y.w * y.w;
     }
-    float* sp = stats + ((r0 / st_rows) * st_ld + c) * 2;
-    red_add_f32x4(sp, s[0], q[0], s[1], q[1]);
-    red_add_f32x4(sp + 4, s[2], q[2], s[3], q[3]);
-}
-
-__global__ void splitk_finish_kernel(const float* __restrict__ acc, const float* __restrict__ bias, const float* __restrict__ rowbias,
-                                     const __nv_bfloat16* __restrict__ residual, void* __restrict__ out, int64_t rows, int C,
-                                     int64_t rows_per_sample, int rb_div, int64_t rb_ld, float alpha, int out_fp32) {
-    pdl_sync();
-    const int V = C >> 2;  // 4 columns per thread
-    const int64_t total = rows * V;
-    for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < total; i += int64_t(gridDim.x) * blockDim.x) {
-        const int64_t r = i / V;
-        const int c = int(i % V) * 4;
-        float4 v = __ldcg(reinterpret_cast<const float4*>(acc + r * C + c));
-        v.x *= alpha; v.y *= alpha; v.z *= alpha; v.w *= alpha;
-        if (bias) {
-            const float4 b = __ldg(reinterpret_cast<const float4*>(bias + c));
-            v.x += b.x; v.y += b.y; v.z += b.z; v.w += b.w;
-        }
-        if (rowbias) {
-            const float4 b = __ldg(reinterpret_cast<const float4*>(rowbias + (r / rows_per_sample / rb_div) * rb_ld + c));
-            v.x += b.x; v.y += b.y; v.z += b.z; v.w += b.w;
-        }
-        if (residual) {
-            const uint2 q = __ldg(reinterpret_cast<const uint2*>(residual + r * C + c));
-            v.x += bf16_lo(q.x); v.y += bf16_hi(q.x); v.z += bf16_lo(q.y); v.w += bf16_hi(q.y);
-        }
-        if (out_fp32) {
-            reinterpret_cast<float4*>(static_cast<float*>(out) + r * C)[c >> 2] = v;
-        } else {
-            uint2 q;
-            q.x = pack_bf16(v.x, v.y);
-            q.y = pack_bf16(v.z, v.w);
-            reinterpret_cast<uint2*>(static_cast<__nv_bfloat16*>(out) + r * C)[c >> 2] = q;
-        }
+    if (stats) {
+        float* sp = stats + ((r0 / st_rows) * st_ld + c) * 2;
+        red_add_f32x4(sp, s[0], q[0], s[1], q[1]);
+        red_add_f32x4(sp + 4, s[2], q[2], s[3], q[3]);
     }
 }
 
@@ -494,25 +466,18 @@ int launch_split(GemmParams& p, bool a_mn, bool b_mn, const T2VEpilogue& e, void
     p.flags = 0;
     set_vec_flag(p);
     if (int r = launch_checked(launch_gemm(p, a_mn, b_mn, st), what)) return r;
-    if (e.stats && e.stats_rows > 0 && e.stats_ld % 2 == 0 && (reinterpret_cast<uintptr_t>(e.stats) & 15u) == 0) {
-        // rows per block: a divisor of the sample's rows, so a block never straddles two samples
-        const int rpb = e.stats_rows % 4 == 0 ? 4 : (e.stats_rows % 2 == 0 ? 2 : 1);
-        const dim3 grid(unsigned((rows + rpb - 1) / rpb), unsigned((C / 4 + 255) / 256));
-        const dim3 block(unsigned(std::min(256, (C / 4 + 31) / 32 * 32)));
-        auto go = [&](auto kern) {
-            return int(launch_pdl(kern, grid, block, 0, st, static_cast<const float*>(e.workspace), e.bias, e.rowbias,
-                                  static_cast<const __nv_bfloat16*>(e.residual), out, rows, C, rows_per_sample,
-                                  e.rowbias_div > 0 ? e.rowbias_div : 1, int64_t(C), e.alpha, e.out_fp32, e.stats, e.stats_ld, e.stats_rows));
-        };
-        const int rc = rpb == 4 ? go(splitk_finish_stats_kernel<4>) : (rpb == 2 ? go(splitk_finish_stats_kernel<2>) : go(splitk_finish_stats_kernel<1>));
-        return launch_checked(rc, what);
-    }
-    const int64_t vec = rows * (C / 4);
-    const int grid = int(std::min<int64_t>((vec + 255) / 256, int64_t(device_sm_count()) * 8));
-    const int rc = int(launch_pdl(splitk_finish_kernel, dim3(grid), dim3(256), 0, st, static_cast<const float*>(e.workspace), e.bias,
-                                  e.rowbias, static_cast<const __nv_bfloat16*>(e.residual), out, rows, C, rows_per_sample,
-                                  e.rowbias_div > 0 ? e.rowbias_div : 1, int64_t(C), e.alpha, e.out_fp32));
-    return launch_checked(rc, what);
+    const bool stats = e.stats && e.stats_rows > 0 && e.stats_ld % 2 == 0 && (reinterpret_cast<uintptr_t>(e.stats) & 15u) == 0;
+    // rows per block: with statistics a divisor of the sample's rows, so that a block never straddles two samples
+    const int rpb = !stats || e.stats_rows % 4 == 0 ? 4 : (e.stats_rows % 2 == 0 ? 2 : 1);
+    const dim3 grid(unsigned((rows + rpb - 1) / rpb), unsigned((C / 4 + 255) / 256));
+    const dim3 block(unsigned(std::min(256, (C / 4 + 31) / 32 * 32)));
+    auto go = [&](auto kern) {
+        return int(launch_pdl(kern, grid, block, 0, st, static_cast<const float*>(e.workspace), e.bias, e.rowbias,
+                              static_cast<const __nv_bfloat16*>(e.residual), out, rows, C, rows_per_sample,
+                              e.rowbias_div > 0 ? e.rowbias_div : 1, int64_t(C), e.alpha, e.out_fp32, stats ? e.stats : nullptr,
+                              e.stats_ld, e.stats_rows));
+    };
+    return launch_checked(rpb == 4 ? go(splitk_finish_kernel<4>) : (rpb == 2 ? go(splitk_finish_kernel<2>) : go(splitk_finish_kernel<1>)), what);
 }
 
 }  // namespace

@@ -79,12 +79,7 @@ __device__ __forceinline__ void acc_ld32(uint32_t arow, uint32_t key, int ch, ui
     }
 }
 
-// Epilogue of one tile (warps 0..7).  Warp w owns accumulator rows 64*(w/4) + 32*(w%2)..+31, i.e. thread <-> output row, and
-// the two warp pairs of a warpgroup split the columns.  Output rows are
-// strided in global memory, so every 32-column chunk goes through a per-warp swizzled staging tile and is moved with
-// 16 bytes per lane covering whole rows (full 64/128-byte segments); the residual comes in the same way.  The per-column
-// bias is fetched with one coalesced load per chunk and broadcast through shared memory.
-// flags of the epilogue fast path: known at compile time (folded away) or only at run time (the catch-all instantiation)
+// flags of the epilogue's chunk body: known at compile time (folded away) or only at run time (the catch-all instantiation)
 template <bool V>
 struct ConstFlag {
     __device__ constexpr operator bool() const { return V; }
@@ -94,13 +89,18 @@ struct RuntimeFlag {
     __device__ constexpr operator bool() const { return v; }
 };
 
+// Epilogue of one tile (warps 0..7).  Warp w owns accumulator rows 64*(w/4) + 32*(w%2)..+31, i.e. thread <-> output row, and
+// the two warp pairs of a warpgroup split the columns.  Output rows are strided in global memory, so every 32-column chunk
+// goes through a per-warp swizzled staging tile and is moved with 16 bytes per lane covering whole rows (full 64/128-byte
+// segments); the residual comes in the same way.  The per-column bias is fetched with one coalesced load per chunk and
+// broadcast through shared memory.  Buffers that are not 16-byte aligned (EPI_VEC clear) take a per-thread scalar path.
+// rowsum_tile: rs_s holds the row sums of operand A for this tile (EPI_ROWSUM_A).
 template <int ESZ>
-__device__ __forceinline__ void epilogue_tile(const GemmParams& p, const TileVars& tile_vars, uint32_t warp, uint32_t lane,
+__device__ __forceinline__ void epilogue_tile(const GemmParams& p, const TileVars& tv, bool rowsum_tile, uint32_t warp, uint32_t lane,
                                               uint32_t acc_s, uint32_t acc_pitch, const float* rs_s, uint8_t* stg_base) {
     constexpr int CPR = ESZ * 2;        // 16-byte chunks per 32-column row: 4 (bf16) or 8 (fp32)
     constexpr int EPC = 16 / ESZ;       // elements per 16-byte chunk
     constexpr int RPI = 32 / CPR;       // rows covered by one warp-wide 16-byte access
-    const uint32_t ew = warp;
     const uint32_t grp = (warp >> 1) & 1u;
     const uint32_t row = (warp >> 2) * 64u + (warp & 1u) * 32u + lane;
     const int32_t rw = static_cast<int32_t>(row) % p.bw;
@@ -108,17 +108,18 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const TileVar
     const int32_t rn = static_cast<int32_t>(row) / (p.bw * p.bh);
     const bool has_bias = p.flags & EPI_BIAS, has_rb = p.flags & EPI_ROWBIAS, has_res = p.flags & EPI_RESIDUAL;
     const bool vec = p.flags & EPI_VEC;
-    const bool has_stats = (p.flags & EPI_STATS) && vec;
+    const bool has_stats = ESZ == 2 && (p.flags & EPI_STATS) && vec;
+    const int32_t col0 = tv.t[0] * p.block_n;
+    // this warp pair's half of the tile's 32-column chunks, without the chunks past the output's last column
     const int nchunks = (p.block_n + 31) >> 5;
     const int c_begin = grp == 0 ? 0 : (nchunks + 1) >> 1;
-    const int c_end = grp == 0 ? (nchunks + 1) >> 1 : nchunks;
-    uint8_t* stg = stg_base + ew * 4096u;                                    // 32 rows x <= 128 B
-    float* sbias = reinterpret_cast<float*>(stg_base + 8 * 4096u) + ew * 32;  // 32 floats per warp
+    const int c_end = min(grp == 0 ? (nchunks + 1) >> 1 : nchunks, (p.ncols - col0 + 31) >> 5);
+    const uint32_t stg_s = smem_u32(stg_base + warp * 4096u);                   // 32 rows x <= 128 B
+    float* sbias = reinterpret_cast<float*>(stg_base + 8 * 4096u) + warp * 32;  // 32 floats per warp
     // swizzled byte offset of logical 16-byte chunk j of row r in a dense [32][n] chunk array
     auto phys = [](int r, int j, int n) { return (r * n + (j ^ (((r * n) >> 3) & (n - 1)))) * 16; };
     const int sr = lane / CPR, sj = lane % CPR;  // (row-in-group, chunk) this lane moves in the coalesced phases
-    // tile-invariant shared-memory addresses of the staging tile (hoisted: the fast path below is straight-line code)
-    const uint32_t stg_s = smem_u32(stg);
+    // tile-invariant shared-memory addresses of the staging tile (hoisted: the chunk body is straight-line code)
     uint32_t w_own[CPR];     // this lane's own row, 16-byte chunk j                     (write after the math)
     uint32_t r_mov[CPR];     // the (row, chunk) this lane moves in the coalesced store   (read)
     uint32_t w_res[4];       // residual staging: row (lane / 4) + 8 i, chunk lane % 4   (write, bf16 rows of 64 B)
@@ -134,331 +135,89 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const TileVar
         r_res[j] = stg_s + phys(static_cast<int>(lane), j, 4);
     }
     const bool alpha_one = p.alpha == 1.0f;
-    {
-        const TileVars& tv = tile_vars;
-        const bool rowsum_tile = (p.flags & EPI_ROWSUM_A) && tv.t[0] == 0 && tv.t[2] == 0 && tv.t[3] == 0 && grp == 0;
-        const int32_t gw = tv.t[1] * p.bw + rw, gh = tv.t[2] * p.bh + rh, gn = tv.t[3] * p.bn + rn;
-        const bool row_ok = (rn < p.bn) && gw < p.W && gh < p.H && gn < p.N;
-        int64_t off = gw * p.ldw + gh * p.ldh + gn * p.ldn;
+    const int32_t gw = tv.t[1] * p.bw + rw, gh = tv.t[2] * p.bh + rh, gn = tv.t[3] * p.bn + rn;
+    const bool row_ok = (rn < p.bn) && gw < p.W && gh < p.H && gn < p.N;
+    int64_t off = gw * p.ldw + gh * p.ldh + gn * p.ldn;
 #pragma unroll
-        for (int i = 0; i < 6; ++i) off += tv.t[i] * p.otc[i];
-        // rows this lane moves in the coalesced phases (constant over the tile's chunks)
-        int64_t off_s[CPR];
-        uint32_t ok_s = 0;
+    for (int i = 0; i < 6; ++i) off += tv.t[i] * p.otc[i];
+    // rows this lane moves in the coalesced phases (constant over the tile's chunks)
+    int64_t off_s[CPR];
+    uint32_t ok_s = 0;
 #pragma unroll
-        for (int i = 0; i < CPR; ++i) {
-            const int r = sr + RPI * i;
-            off_s[i] = __shfl_sync(0xffffffffu, off, r);
-            ok_s |= (__shfl_sync(0xffffffffu, row_ok ? 1u : 0u, r) & 1u) << i;
+    for (int i = 0; i < CPR; ++i) {
+        const int r = sr + RPI * i;
+        off_s[i] = __shfl_sync(0xffffffffu, off, r);
+        ok_s |= (__shfl_sync(0xffffffffu, row_ok ? 1u : 0u, r) & 1u) << i;
+    }
+    // every row of this warp inside the output: full chunks run without per-row predicates
+    const bool all_rows = vec && __all_sync(0xffffffffu, row_ok);
+    // GroupNorm statistics: frame of this lane's segment (taken from the segment's first row, which is in bounds
+    // whenever any row of the segment is)
+    int64_t st_off = 0;
+    uint32_t okmask = 0;
+    if (has_stats) {
+        const int32_t fr = (gw * p.st_cw + gh * p.st_ch + gn * p.st_cn) / p.st_div;
+        st_off = int64_t(__shfl_sync(0xffffffffu, fr, lane & ~uint32_t(p.st_seg - 1))) * p.st_ld;
+        okmask = __ballot_sync(0xffffffffu, row_ok);
+    }
+    // ---- software pipeline of the epilogue's global loads.  Per-column additive terms (bias, and the time-embedding row
+    // when every row of this warp takes the same one) are fetched two chunks ahead, the residual tile one chunk ahead;
+    // the first of them are issued BEFORE the wait for the accumulator, so their latency hides behind the main loop.
+    // (every lane takes part in the shuffle: it must not sit behind a short-circuit that depends on row_ok)
+    // The row is taken from the warp's first IN-BOUNDS lane: an out-of-bounds lane (frames beyond N in the last tile) would
+    // name a row past the end of the time-embedding matrix.  A warp without any valid row folds nothing.
+    const int32_t rb_row = has_rb ? gn / p.rb_div : 0;
+    const uint32_t ok_lanes = __ballot_sync(0xffffffffu, row_ok);
+    const int32_t rb_first = __shfl_sync(0xffffffffu, rb_row, ok_lanes ? __ffs(ok_lanes) - 1 : 0);
+    const bool rb_same = !row_ok || rb_row == rb_first;
+    const bool rb_uniform = has_rb && vec && ok_lanes != 0u && __all_sync(0xffffffffu, rb_same);
+    const float* rb_base = has_rb ? p.rowbias + static_cast<int64_t>(rb_first) * p.rb_ld : nullptr;
+    const bool colterm = has_bias || rb_uniform;   // a per-column term, broadcast through sbias
+    const bool row_rb = has_rb && !rb_uniform;     // a time-embedding row per output row
+    auto load_colterm = [&](int ch) {
+        const int32_t c = col0 + ch * 32 + static_cast<int32_t>(lane);
+        float b = 0.f;
+        if (static_cast<int32_t>(lane) < min(32, min(p.block_n - ch * 32, p.ncols - (col0 + ch * 32)))) {
+            if (has_bias) b = __ldg(p.bias + c);
+            if (rb_uniform) b += __ldg(rb_base + c);
         }
-        const int32_t col0 = tv.t[0] * p.block_n;
-        // every row of this warp inside the output: the common case runs without per-row predicates
-        const bool all_rows = vec && __all_sync(0xffffffffu, row_ok);
-        // GroupNorm statistics: frame of this lane's segment (taken from the segment's first row, which is in bounds
-        // whenever any row of the segment is)
-        int64_t st_off = 0;
-        uint32_t okmask = 0;
-        if (has_stats) {
-            const int32_t fr = (gw * p.st_cw + gh * p.st_ch + gn * p.st_cn) / p.st_div;
-            st_off = int64_t(__shfl_sync(0xffffffffu, fr, lane & ~uint32_t(p.st_seg - 1))) * p.st_ld;
-            okmask = __ballot_sync(0xffffffffu, row_ok);
+        return b;
+    };
+    // The residual is prefetched only when every row is in bounds, and only for a full-width chunk: only a full chunk uses it
+    const bool res_pref = all_rows && has_res;
+    const __nv_bfloat16* res_lane = static_cast<const __nv_bfloat16*>(p.residual) + (lane & 3) * 8;
+    int64_t off_q[4];   // residual rows this lane fetches: (lane / 4) + 8 i
+#pragma unroll
+    for (int i = 0; i < 4; ++i) off_q[i] = __shfl_sync(0xffffffffu, off, (lane >> 2) + 8 * i);
+    auto load_res = [&](int ch, uint4 (&q)[4]) {
+        const int32_t c = col0 + ch * 32;
+        if (min(p.block_n - ch * 32, p.ncols - c) >= 32) {
+#pragma unroll
+            for (int i = 0; i < 4; ++i) q[i] = __ldg(reinterpret_cast<const uint4*>(res_lane + off_q[i] + c));
         }
-        // ---- software pipeline of the epilogue's global loads.  Per-column additive terms (bias, and the time-embedding row
-        // when every row of this warp takes the same one) are fetched two chunks ahead, the residual tile one chunk ahead;
-        // the first of them are issued BEFORE the wait for the accumulator, so their latency hides behind the main loop.
-        // (every lane takes part in the shuffle: it must not sit behind a short-circuit that depends on row_ok)
-        // The row is taken from the warp's first IN-BOUNDS lane: an out-of-bounds lane (frames beyond N in the last tile) would
-        // name a row past the end of the time-embedding matrix.  A warp without any valid row folds nothing.
-        const int32_t rb_row = has_rb ? gn / p.rb_div : 0;
-        const uint32_t ok_lanes = __ballot_sync(0xffffffffu, row_ok);
-        const int32_t rb_first = __shfl_sync(0xffffffffu, rb_row, ok_lanes ? __ffs(ok_lanes) - 1 : 0);
-        const bool rb_same = !row_ok || rb_row == rb_first;
-        const bool rb_uniform = has_rb && vec && ok_lanes != 0u && __all_sync(0xffffffffu, rb_same);
-        const float* rb_base = has_rb ? p.rowbias + static_cast<int64_t>(rb_first) * p.rb_ld : nullptr;
-        auto load_colterm = [&](int ch) {
-            const int32_t c = col0 + ch * 32 + static_cast<int32_t>(lane);
-            float b = 0.f;
-            if (static_cast<int32_t>(lane) < min(32, min(p.block_n - ch * 32, p.ncols - (col0 + ch * 32)))) {
-                if (has_bias) b = __ldg(p.bias + c);
-                if (rb_uniform) b += __ldg(rb_base + c);
-            }
-            return b;
-        };
-        const bool res_pref = all_rows && has_res;
-        const __nv_bfloat16* res_lane = static_cast<const __nv_bfloat16*>(p.residual) + (lane & 3) * 8;
-        int64_t off_q[4];   // residual rows this lane fetches: (lane / 4) + 8 i
-#pragma unroll
-        for (int i = 0; i < 4; ++i) off_q[i] = __shfl_sync(0xffffffffu, off, (lane >> 2) + 8 * i);
-        auto load_res = [&](int ch, uint4 (&q)[4]) {
-            const int32_t c = col0 + ch * 32;
-            if (min(p.block_n - ch * 32, p.ncols - c) >= 32) {
-#pragma unroll
-                for (int i = 0; i < 4; ++i) q[i] = __ldg(reinterpret_cast<const uint4*>(res_lane + off_q[i] + c));
-            }
-        };
-        float bq0 = 0.f, bq1 = 0.f;
-        uint4 rq[4] = {};
-        if (c_begin < c_end) bq0 = load_colterm(c_begin);
-        if (c_begin + 1 < c_end) bq1 = load_colterm(c_begin + 1);
-        if (res_pref && c_begin < c_end) load_res(c_begin, rq);
-        const uint32_t arow = acc_s + row * acc_pitch * 4u, akey = acc_swz(row);
-        uint32_t acc[32];
-        if (c_begin < c_end) acc_ld32(arow, akey, c_begin, acc);  // chunk ch+1 is read while chunk ch goes out to global memory
-        for (int ch = c_begin; ch < c_end; ++ch) {
-            const int32_t col = col0 + ch * 32;
-            const int32_t cvalid = min(32, min(p.block_n - ch * 32, p.ncols - col));  // valid columns of this chunk
-            __syncwarp();
-            const float bcur = bq0;          // this chunk's per-column term; keep the pipeline two chunks deep
-            bq0 = bq1;
-            if (ch + 2 < c_end) bq1 = load_colterm(ch + 2);
-            const bool colterm = has_bias || rb_uniform;
-            if (all_rows && cvalid == 32) {
-                // ---- fast path: a full 32 x 32 chunk, every row in bounds.  The body is instantiated per combination of
-                // (column term, residual, statistics, alpha, per-row time embedding) so that each instantiation is
-                // straight-line code without flag tests (in a flag-driven version a third of the instructions per chunk
-                // were predicate bookkeeping).
-                auto fast = [&](auto kCol, auto kRes, auto kStats, auto kAlpha, auto kRowRb) {
-                    // each flag is a ConstFlag (folded at compile time) or a RuntimeFlag (the catch-all instantiation)
-                    const bool COL = kCol, RES = kRes, STATS = kStats, ALPHA = kAlpha, ROWRB = kRowRb;
-                    if (COL) sbias[lane] = bcur;
-                    if (RES) {   // residual (prefetched one chunk ago): registers -> staging, then fetch the next chunk's
-#pragma unroll
-                        for (int i = 0; i < 4; ++i) sts128(w_res[i], rq[i]);
-                        if (ch + 1 < c_end) load_res(ch + 1, rq);
-                    }
-                    float* v = reinterpret_cast<float*>(acc);   // in place: the accumulator registers are not reloaded until the
-                    if (ALPHA) {                      // values have been packed into the staging tile
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) v[j] *= p.alpha;
-                    }
-                    if (COL || RES) __syncwarp();
-                    if (COL) {
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            const float4 b = *reinterpret_cast<const float4*>(sbias + 4 * j);  // shared-memory broadcast
-                            v[4 * j] += b.x; v[4 * j + 1] += b.y; v[4 * j + 2] += b.z; v[4 * j + 3] += b.w;
-                        }
-                    }
-                    if (ROWRB) {
-                        const float4* b4 = reinterpret_cast<const float4*>(p.rowbias + (gn / p.rb_div) * p.rb_ld + col);
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            const float4 b = __ldg(b4 + j);
-                            v[4 * j] += b.x; v[4 * j + 1] += b.y; v[4 * j + 2] += b.z; v[4 * j + 3] += b.w;
-                        }
-                    }
-                    if (RES) {
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            const uint4 q = lds128(r_res[j]);
-                            v[8 * j + 0] += bf16_lo(q.x); v[8 * j + 1] += bf16_hi(q.x);
-                            v[8 * j + 2] += bf16_lo(q.y); v[8 * j + 3] += bf16_hi(q.y);
-                            v[8 * j + 4] += bf16_lo(q.z); v[8 * j + 5] += bf16_hi(q.z);
-                            v[8 * j + 6] += bf16_lo(q.w); v[8 * j + 7] += bf16_hi(q.w);
-                        }
-                        __syncwarp();
-                    }
-                    if constexpr (ESZ == 2) {
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            uint4 q;
-                            q.x = pack_bf16(v[8 * j + 0], v[8 * j + 1]);
-                            q.y = pack_bf16(v[8 * j + 2], v[8 * j + 3]);
-                            q.z = pack_bf16(v[8 * j + 4], v[8 * j + 5]);
-                            q.w = pack_bf16(v[8 * j + 6], v[8 * j + 7]);
-                            sts128(w_own[j], q);
-                        }
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < CPR; ++j) sts128(w_own[j], make_uint4(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]));
-                    }
-                    if (ch + 1 < c_end) acc_ld32(arow, akey, ch + 1, acc);   // next chunk
-                    __syncwarp();
-                    if (ESZ == 2 && STATS) {   // GroupNorm statistics of the staged bf16 tile (see the general path below)
-                        const uint32_t half = lane >> 4, cw = lane & 15u;
-                        float s0 = 0.f, q0 = 0.f, s1 = 0.f, q1 = 0.f;
-#pragma unroll
-                        for (int i = 0; i < 16; ++i) {
-                            const int r = half ? 16 + ((i + 1) & 15) : i;
-                            const uint32_t w = lds32(stg_s + phys(r, int(cw >> 2), 4) + (cw & 3u) * 4u);
-                            const float lo = bf16_lo(w), hi = bf16_hi(w);
-                            s0 += lo; q0 += lo * lo;
-                            s1 += hi; q1 += hi * hi;
-                        }
-                        if (p.st_seg == 32) {
-                            s0 += __shfl_xor_sync(0xffffffffu, s0, 16); q0 += __shfl_xor_sync(0xffffffffu, q0, 16);
-                            s1 += __shfl_xor_sync(0xffffffffu, s1, 16); q1 += __shfl_xor_sync(0xffffffffu, q1, 16);
-                        }
-                        if (p.st_seg == 16 || half == 0) red_add_f32x4(p.stats + (st_off + col + 2 * cw) * 2, s0, q0, s1, q1);
-                    }
-                    // staging -> global: 16 bytes per lane, whole row segments
-                    char* ob = static_cast<char*>(p.out) + (static_cast<int64_t>(col) + sj * EPC) * ESZ;
-#pragma unroll
-                    for (int i = 0; i < CPR; ++i) {
-                        const uint4 q = lds128(r_mov[i]);
-                        char* o = ob + off_s[i] * ESZ;
-                        if (ESZ == 2 || p.out_mode == OUT_F32) {
-                            *reinterpret_cast<uint4*>(o) = q;
-                        } else {
-                            red_add_f32x4(reinterpret_cast<float*>(o), __uint_as_float(q.x), __uint_as_float(q.y), __uint_as_float(q.z),
-                                          __uint_as_float(q.w));
-                        }
-                    }
-                };
-                using T = ConstFlag<true>;
-                using F = ConstFlag<false>;
-                const bool row_rb = has_rb && !rb_uniform;
-                const int key = (colterm ? 1 : 0) | (has_res ? 2 : 0) | ((ESZ == 2 && has_stats) ? 4 : 0) | (alpha_one ? 0 : 8) | (row_rb ? 16 : 0);
-                switch (key) {
-                    case 0: fast(F{}, F{}, F{}, F{}, F{}); break;     // plain (dgrad, attention products)
-                    case 1: fast(T{}, F{}, F{}, F{}, F{}); break;     // bias (+ folded time embedding)
-                    case 2: fast(F{}, T{}, F{}, F{}, F{}); break;     // residual
-                    case 3: fast(T{}, T{}, F{}, F{}, F{}); break;     // bias + residual
-                    case 4: fast(F{}, F{}, T{}, F{}, F{}); break;     // ... the same with GroupNorm statistics
-                    case 5: fast(T{}, F{}, T{}, F{}, F{}); break;
-                    case 6: fast(F{}, T{}, T{}, F{}, F{}); break;
-                    case 7: fast(T{}, T{}, T{}, F{}, F{}); break;
-                    default: {                                         // alpha != 1 / per-row time embedding: rare, runtime flags
-                        using R = RuntimeFlag;
-                        fast(R{colterm}, R{has_res}, R{ESZ == 2 && has_stats}, R{!alpha_one}, R{row_rb});
-                        break;
-                    }
-                }
-                continue;
-            }
-            if (res_pref && ch + 1 < c_end) load_res(ch + 1, rq);   // keep the residual pipeline primed for a following fast chunk
-            const float bval = bcur;   // bias (+ the warp-uniform time-embedding row) of this chunk, fetched two chunks ago
-            if (vec && has_res && cvalid > 0) {         // residual: coalesced global -> staging (bf16, 4 chunks per row)
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    const int r = (lane >> 2) + 8 * i, j = lane & 3;
-                    const int64_t off_r = __shfl_sync(0xffffffffu, off, r);
-                    const bool ok_r = __shfl_sync(0xffffffffu, row_ok ? 1 : 0, r);
-                    uint4 q = make_uint4(0, 0, 0, 0);
-                    if (ok_r && j * 8 + 8 <= cvalid)
-                        q = __ldg(reinterpret_cast<const uint4*>(static_cast<const __nv_bfloat16*>(p.residual) + off_r + col + j * 8));
-                    *reinterpret_cast<uint4*>(stg + phys(r, j, 4)) = q;
-                }
-            }
-            sbias[lane] = bval;
-            float v[32];
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(acc[j]) * p.alpha;
-            if (ch + 1 < c_end) acc_ld32(arow, akey, ch + 1, acc);
-            __syncwarp();
-            if (cvalid <= 0) continue;
-            if (vec) {
-                if (colterm) {
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        const float4 b = *reinterpret_cast<const float4*>(sbias + 4 * j);  // shared-memory broadcast
-                        v[4 * j] += b.x; v[4 * j + 1] += b.y; v[4 * j + 2] += b.z; v[4 * j + 3] += b.w;
-                    }
-                }
-                if (has_rb && !rb_uniform && row_ok) {
-                    const float4* b4 = reinterpret_cast<const float4*>(p.rowbias + (gn / p.rb_div) * p.rb_ld + col);
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        if (j * 4 + 4 <= cvalid) {
-                            const float4 b = __ldg(b4 + j);
-                            v[4 * j] += b.x; v[4 * j + 1] += b.y; v[4 * j + 2] += b.z; v[4 * j + 3] += b.w;
-                        }
-                    }
-                }
-                if (has_res) {
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        const uint4 q = *reinterpret_cast<const uint4*>(stg + phys(lane, j, 4));
-                        v[8 * j + 0] += bf16_lo(q.x); v[8 * j + 1] += bf16_hi(q.x);
-                        v[8 * j + 2] += bf16_lo(q.y); v[8 * j + 3] += bf16_hi(q.y);
-                        v[8 * j + 4] += bf16_lo(q.z); v[8 * j + 5] += bf16_hi(q.z);
-                        v[8 * j + 6] += bf16_lo(q.w); v[8 * j + 7] += bf16_hi(q.w);
-                    }
-                    __syncwarp();
-                }
-                // own row -> staging
-                if (ESZ == 2) {
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        uint4 q;
-                        q.x = pack_bf16(v[8 * j + 0], v[8 * j + 1]);
-                        q.y = pack_bf16(v[8 * j + 2], v[8 * j + 3]);
-                        q.z = pack_bf16(v[8 * j + 4], v[8 * j + 5]);
-                        q.w = pack_bf16(v[8 * j + 6], v[8 * j + 7]);
-                        *reinterpret_cast<uint4*>(stg + phys(lane, j, 4)) = q;
-                    }
-                } else {
-#pragma unroll
-                    for (int j = 0; j < 8; ++j)
-                        *reinterpret_cast<float4*>(stg + phys(lane, j, 8)) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-                }
-                __syncwarp();
-                if (ESZ == 2 && has_stats) {
-                    // GroupNorm statistics of the tile just staged (the bf16 values the consumer will read): lanes 0-15 walk
-                    // rows 0-15, lanes 16-31 rows 16-31 (staggered by one row so the two halves hit different banks), each lane
-                    // owns the column pair (2c, 2c+1), c = lane % 16.  16-row segments: every half is one frame; 32-row
-                    // segments: the halves are combined with one shuffle.
-                    const uint32_t half = lane >> 4, cw = lane & 15u;
-                    float s0 = 0.f, q0 = 0.f, s1 = 0.f, q1 = 0.f;
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) {
-                        const int r = half ? 16 + ((i + 1) & 15) : i;
-                        const uint32_t w = *reinterpret_cast<const uint32_t*>(stg + phys(r, int(cw >> 2), 4) + (cw & 3u) * 4u);
-                        if ((okmask >> r) & 1u) {
-                            const float lo = bf16_lo(w), hi = bf16_hi(w);
-                            s0 += lo; q0 += lo * lo;
-                            s1 += hi; q1 += hi * hi;
-                        }
-                    }
-                    if (p.st_seg == 32) {
-                        s0 += __shfl_xor_sync(0xffffffffu, s0, 16); q0 += __shfl_xor_sync(0xffffffffu, q0, 16);
-                        s1 += __shfl_xor_sync(0xffffffffu, s1, 16); q1 += __shfl_xor_sync(0xffffffffu, q1, 16);
-                    }
-                    // a segment without a valid row has no frame (its offset is meaningless): it contributes nothing
-                    const bool any_row = p.st_seg == 16 ? ((okmask >> (half * 16u)) & 0xFFFFu) != 0u : okmask != 0u;
-                    if (any_row && (p.st_seg == 16 || half == 0) && int(2 * cw) < cvalid)
-                        red_add_f32x4(p.stats + (st_off + col + 2 * cw) * 2, s0, q0, s1, q1);
-                }
-                // staging -> global: 16 bytes per lane, whole row segments
-                const int nval = cvalid - sj * EPC;  // valid elements in this lane's chunk
-#pragma unroll
-                for (int i = 0; i < CPR; ++i) {
-                    if (!((ok_s >> i) & 1u) || nval <= 0) continue;
-                    const int r = sr + RPI * i;
-                    const uint4 q = *reinterpret_cast<const uint4*>(stg + phys(r, sj, CPR));
-                    const int64_t o = off_s[i] + col + sj * EPC;
-                    if (nval >= EPC) {
-                        if (ESZ == 2) {
-                            *reinterpret_cast<uint4*>(static_cast<__nv_bfloat16*>(p.out) + o) = q;
-                        } else if (p.out_mode == OUT_F32) {
-                            *reinterpret_cast<uint4*>(static_cast<float*>(p.out) + o) = q;
-                        } else {
-                            red_add_f32x4(static_cast<float*>(p.out) + o, __uint_as_float(q.x), __uint_as_float(q.y), __uint_as_float(q.z),
-                                          __uint_as_float(q.w));
-                        }
-                    } else {  // ragged last chunk: element-wise
-                        // (static indexing only: a runtime-indexed register array would be demoted to local memory)
-                        const uint32_t w4[4] = {q.x, q.y, q.z, q.w};
-#pragma unroll
-                        for (int e = 0; e < EPC; ++e) {
-                            if (e >= nval) break;
-                            if (ESZ == 2) {
-                                const uint32_t h = (w4[e >> 1] >> ((e & 1) * 16)) & 0xFFFFu;
-                                reinterpret_cast<uint16_t*>(p.out)[o + e] = static_cast<uint16_t>(h);
-                            } else if (p.out_mode == OUT_F32) {
-                                static_cast<float*>(p.out)[o + e] = __uint_as_float(w4[e & 3]);
-                            } else {
-                                atomicAdd(static_cast<float*>(p.out) + o + e, __uint_as_float(w4[e & 3]));
-                            }
-                        }
-                    }
-                }
-            } else if (row_ok) {
-                // unaligned buffers: per-thread scalar path
+    };
+    float bq0 = 0.f, bq1 = 0.f;
+    uint4 rq[4] = {};
+    if (c_begin < c_end) bq0 = load_colterm(c_begin);
+    if (c_begin + 1 < c_end) bq1 = load_colterm(c_begin + 1);
+    if (res_pref && c_begin < c_end) load_res(c_begin, rq);
+    const uint32_t arow = acc_s + row * acc_pitch * 4u, akey = acc_swz(row);
+    uint32_t acc[32];
+    if (c_begin < c_end) acc_ld32(arow, akey, c_begin, acc);  // chunk ch+1 is read while chunk ch goes out to global memory
+    for (int ch = c_begin; ch < c_end; ++ch) {
+        const int32_t col = col0 + ch * 32;
+        const int32_t cvalid = min(32, min(p.block_n - ch * 32, p.ncols - col));  // valid columns of this chunk, >= 1
+        __syncwarp();
+        const float bcur = bq0;          // this chunk's per-column term; keep the pipeline two chunks deep
+        bq0 = bq1;
+        if (ch + 2 < c_end) bq1 = load_colterm(ch + 2);
+        if (!vec) {
+            // unaligned buffers: each thread writes its own row, element by element
+            if (row_ok) {
 #pragma unroll
                 for (int j = 0; j < 32; ++j) {
                     if (j >= cvalid) break;
-                    float x = v[j];
+                    float x = __uint_as_float(acc[j]) * p.alpha;
                     if (has_bias) x += p.bias[col + j];
                     if (has_rb) x += p.rowbias[(gn / p.rb_div) * p.rb_ld + col + j];
                     if (has_res) x += __bfloat162float(static_cast<const __nv_bfloat16*>(p.residual)[off + col + j]);
@@ -467,13 +226,159 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const TileVar
                     else atomicAdd(static_cast<float*>(p.out) + off + col + j, x);
                 }
             }
+            if (ch + 1 < c_end) acc_ld32(arow, akey, ch + 1, acc);
+            continue;
         }
-        if (rowsum_tile) {
-            // row sums of operand A (weight gradient: the bias gradient).  Both warp pairs of a warpgroup see the same rows (they
-            // split the columns) - pair 0 alone adds them.
-            if (row_ok) atomicAdd(p.rowsum + gw, rs_s[row]);
+        // ---- one chunk: alpha, column term, per-row time embedding, residual, packing, statistics, coalesced store.  The
+        // body is instantiated per combination of (full chunk, column term, residual, statistics, alpha, per-row time
+        // embedding) so that the common full chunks run straight-line code without flag tests (in a flag-driven version a
+        // third of the instructions per chunk were predicate bookkeeping).  A full chunk is 32 x 32 with every row of the
+        // warp in bounds; any other chunk applies the row and column predicates.
+        auto body = [&](auto kFull, auto kCol, auto kRes, auto kStats, auto kAlpha, auto kRowRb) {
+            // each flag is a ConstFlag (folded at compile time) or a RuntimeFlag (the catch-all instantiation)
+            const bool FULL = kFull, COL = kCol, RES = kRes, STATS = kStats, ALPHA = kAlpha, ROWRB = kRowRb;
+            if (COL) sbias[lane] = bcur;
+            if (RES) {   // residual -> staging: a full chunk's was prefetched one chunk ago, any other is loaded here
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    uint4 q = rq[i];
+                    if (!FULL) {
+                        const bool ok_r = __shfl_sync(0xffffffffu, row_ok ? 1 : 0, (lane >> 2) + 8 * i);
+                        q = make_uint4(0, 0, 0, 0);
+                        if (ok_r && (lane & 3) * 8 + 8 <= cvalid) q = __ldg(reinterpret_cast<const uint4*>(res_lane + off_q[i] + col));
+                    }
+                    sts128(w_res[i], q);
+                }
+                if ((FULL || res_pref) && ch + 1 < c_end) load_res(ch + 1, rq);
+            }
+            float* v = reinterpret_cast<float*>(acc);   // in place: the accumulator registers are not reloaded until the
+            if (ALPHA) {                                  // values have been packed into the staging tile
+#pragma unroll
+                for (int j = 0; j < 32; ++j) v[j] *= p.alpha;
+            }
+            if (COL || RES) __syncwarp();
+            if (COL) {
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    const float4 b = *reinterpret_cast<const float4*>(sbias + 4 * j);  // shared-memory broadcast
+                    v[4 * j] += b.x; v[4 * j + 1] += b.y; v[4 * j + 2] += b.z; v[4 * j + 3] += b.w;
+                }
+            }
+            if (ROWRB && (FULL || row_ok)) {
+                const float4* b4 = reinterpret_cast<const float4*>(p.rowbias + (gn / p.rb_div) * p.rb_ld + col);
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    if (FULL || j * 4 + 4 <= cvalid) {
+                        const float4 b = __ldg(b4 + j);
+                        v[4 * j] += b.x; v[4 * j + 1] += b.y; v[4 * j + 2] += b.z; v[4 * j + 3] += b.w;
+                    }
+                }
+            }
+            if (RES) {
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const uint4 q = lds128(r_res[j]);
+                    v[8 * j + 0] += bf16_lo(q.x); v[8 * j + 1] += bf16_hi(q.x);
+                    v[8 * j + 2] += bf16_lo(q.y); v[8 * j + 3] += bf16_hi(q.y);
+                    v[8 * j + 4] += bf16_lo(q.z); v[8 * j + 5] += bf16_hi(q.z);
+                    v[8 * j + 6] += bf16_lo(q.w); v[8 * j + 7] += bf16_hi(q.w);
+                }
+                __syncwarp();
+            }
+            // own row -> staging
+            if constexpr (ESZ == 2) {
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    uint4 q;
+                    q.x = pack_bf16(v[8 * j + 0], v[8 * j + 1]);
+                    q.y = pack_bf16(v[8 * j + 2], v[8 * j + 3]);
+                    q.z = pack_bf16(v[8 * j + 4], v[8 * j + 5]);
+                    q.w = pack_bf16(v[8 * j + 6], v[8 * j + 7]);
+                    sts128(w_own[j], q);
+                }
+            } else {
+#pragma unroll
+                for (int j = 0; j < CPR; ++j) sts128(w_own[j], make_uint4(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]));
+            }
+            if (ch + 1 < c_end) acc_ld32(arow, akey, ch + 1, acc);   // next chunk
+            __syncwarp();
+            if (ESZ == 2 && STATS) {
+                // GroupNorm statistics of the tile just staged (the bf16 values the consumer will read): lanes 0-15 walk
+                // rows 0-15, lanes 16-31 rows 16-31 (staggered by one row so the two halves hit different banks), each lane
+                // owns the column pair (2c, 2c+1), c = lane % 16.  16-row segments: every half is one frame; 32-row
+                // segments: the halves are combined with one shuffle.
+                const uint32_t half = lane >> 4, cw = lane & 15u;
+                float s0 = 0.f, q0 = 0.f, s1 = 0.f, q1 = 0.f;
+#pragma unroll
+                for (int i = 0; i < 16; ++i) {
+                    const int r = half ? 16 + ((i + 1) & 15) : i;
+                    const uint32_t w = lds32(stg_s + phys(r, int(cw >> 2), 4) + (cw & 3u) * 4u);
+                    if (FULL || ((okmask >> r) & 1u)) {
+                        const float lo = bf16_lo(w), hi = bf16_hi(w);
+                        s0 += lo; q0 += lo * lo;
+                        s1 += hi; q1 += hi * hi;
+                    }
+                }
+                if (p.st_seg == 32) {
+                    s0 += __shfl_xor_sync(0xffffffffu, s0, 16); q0 += __shfl_xor_sync(0xffffffffu, q0, 16);
+                    s1 += __shfl_xor_sync(0xffffffffu, s1, 16); q1 += __shfl_xor_sync(0xffffffffu, q1, 16);
+                }
+                // a segment without a valid row has no frame (its offset is meaningless): it contributes nothing
+                const bool any_row = FULL || (p.st_seg == 16 ? ((okmask >> (half * 16u)) & 0xFFFFu) != 0u : okmask != 0u);
+                if (any_row && (p.st_seg == 16 || half == 0) && (FULL || int(2 * cw) < cvalid))
+                    red_add_f32x4(p.stats + (st_off + col + 2 * cw) * 2, s0, q0, s1, q1);
+            }
+            // staging -> global: 16 bytes per lane, whole row segments
+            const int nval = cvalid - sj * EPC;  // valid elements in this lane's 16-byte chunk
+            char* ob = static_cast<char*>(p.out) + (static_cast<int64_t>(col) + sj * EPC) * ESZ;
+#pragma unroll
+            for (int i = 0; i < CPR; ++i) {
+                if (!FULL && (!((ok_s >> i) & 1u) || nval <= 0)) continue;
+                const uint4 q = lds128(r_mov[i]);
+                char* o = ob + off_s[i] * ESZ;
+                if (FULL || nval >= EPC) {
+                    if (ESZ == 2 || p.out_mode == OUT_F32) {
+                        *reinterpret_cast<uint4*>(o) = q;
+                    } else {
+                        red_add_f32x4(reinterpret_cast<float*>(o), __uint_as_float(q.x), __uint_as_float(q.y), __uint_as_float(q.z),
+                                      __uint_as_float(q.w));
+                    }
+                } else {  // ragged last chunk: element-wise
+                    // (static indexing only: a runtime-indexed register array would be demoted to local memory)
+                    const uint32_t w4[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+                    for (int e = 0; e < EPC; ++e) {
+                        if (e >= nval) break;
+                        if (ESZ == 2) reinterpret_cast<uint16_t*>(o)[e] = static_cast<uint16_t>((w4[e >> 1] >> ((e & 1) * 16)) & 0xFFFFu);
+                        else if (p.out_mode == OUT_F32) reinterpret_cast<float*>(o)[e] = __uint_as_float(w4[e & 3]);
+                        else atomicAdd(reinterpret_cast<float*>(o) + e, __uint_as_float(w4[e & 3]));
+                    }
+                }
+            }
+        };
+        using T = ConstFlag<true>;
+        using F = ConstFlag<false>;
+        const bool full = all_rows && cvalid == 32;
+        const int key = full && alpha_one && !row_rb ? (colterm ? 1 : 0) | (has_res ? 2 : 0) | (has_stats ? 4 : 0) : 8;
+        switch (key) {
+            case 0: body(T{}, F{}, F{}, F{}, F{}, F{}); break;     // plain (dgrad, attention products)
+            case 1: body(T{}, T{}, F{}, F{}, F{}, F{}); break;     // bias (+ folded time embedding)
+            case 2: body(T{}, F{}, T{}, F{}, F{}, F{}); break;     // residual
+            case 3: body(T{}, T{}, T{}, F{}, F{}, F{}); break;     // bias + residual
+            case 4: body(T{}, F{}, F{}, T{}, F{}, F{}); break;     // ... the same with GroupNorm statistics
+            case 5: body(T{}, T{}, F{}, T{}, F{}, F{}); break;
+            case 6: body(T{}, F{}, T{}, T{}, F{}, F{}); break;
+            case 7: body(T{}, T{}, T{}, T{}, F{}, F{}); break;
+            default: {                                              // alpha != 1 / per-row time embedding / ragged chunk
+                using R = RuntimeFlag;
+                body(R{full}, R{colterm}, R{has_res}, R{has_stats}, R{!alpha_one}, R{row_rb});
+                break;
+            }
         }
     }
+    // row sums of operand A (weight gradient: the bias gradient).  Both warp pairs of a warpgroup see the same rows (they
+    // split the columns) - pair 0 alone adds them.
+    if (rowsum_tile && grp == 0 && row_ok) atomicAdd(p.rowsum + gw, rs_s[row]);
 }
 
 // One 64 x BN x 16 step of a consumer warpgroup.
@@ -681,8 +586,8 @@ __global__ void __launch_bounds__(kNumThreads, 1) gemm_tc_kernel(const __grid_co
                 }
             }
             named_bar_sync(1 + wg, 128);
-            if (p.out_mode == OUT_BF16) epilogue_tile<2>(p, tv, warp, lane, acc_s, acc_pitch, rs_s, stg_base);
-            else epilogue_tile<4>(p, tv, warp, lane, acc_s, acc_pitch, rs_s, stg_base);
+            if (p.out_mode == OUT_BF16) epilogue_tile<2>(p, tv, rowsum_tile, warp, lane, acc_s, acc_pitch, rs_s, stg_base);
+            else epilogue_tile<4>(p, tv, rowsum_tile, warp, lane, acc_s, acc_pitch, rs_s, stg_base);
         }
     }
 }
