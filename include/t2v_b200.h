@@ -297,6 +297,20 @@ int t2v_adamw_prepare(const float* hp_in, float* hp, int32_t n_sets, int64_t* st
 int t2v_adamw_chunks(float* p, float* g, const void* g_bf16, float* m, float* v, void* shadow_bf16, int64_t n_shadow, const int64_t* chunks,
                      int32_t n_chunks, const float* hp, int32_t zero_grad, void* stream);
 
+/* Blockwise 8-bit AdamW (optim.AdamW8bit): the same update, with the moments of large tensors kept as uint8 codes into two
+ * 256-entry maps (qmaps[0..255] signed for m, qmaps[256..511] unsigned for v) times one fp32 absmax per 256-element block.
+ * chunks: n_chunks int64 rows (arena offset, length, state offset, bits), each inside one tensor and at most 64 K elements.
+ *   bits 32: m32 / v32 (fp32) at the state offset, exactly t2v_adamw_chunks' update.
+ *   bits 8:  code_m / code_v (uint8) at the state offset (a multiple of 256), absmax_m / absmax_v at state offset / 256; the
+ *            length is a multiple of 256 except in a tensor's last row (a multiple of 64).  Per element: dequantise
+ *            (map[code] * absmax), update as t2v_adamw_chunks with the fp32 moments, then per block absmax = max |moment| and
+ *            code = the smallest i with moment / absmax <= 0.5f * (map[i] + map[i+1]); a block whose absmax is 0 stores the
+ *            code of 0.0.
+ * hp, g_bf16, shadow_bf16, n_shadow and zero_grad as for t2v_adamw_chunks.                                                */
+int t2v_adamw8bit_chunks(float* p, float* g, const void* g_bf16, void* shadow_bf16, int64_t n_shadow, const int64_t* chunks, int32_t n_chunks,
+                         const float* hp, const float* qmaps, float* m32, float* v32, void* code_m, void* code_v, float* absmax_m,
+                         float* absmax_v, int32_t zero_grad, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

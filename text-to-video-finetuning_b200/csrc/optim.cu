@@ -8,6 +8,8 @@
 //   update   reads p, g, m, v, writes p, m, v, the bf16 compute shadow of p (kernel layout == master layout, so the
 //            per-step cast kernel disappears) and zero into g (so the per-step gradient memset disappears)  34 B / param
 // HBM-bound; algorithmic bytes = 38 per trainable parameter with clipping, 34 without.
+// The blockwise 8-bit update (adamw8bit_chunks) replaces the 16 B of fp32 m, v traffic by 2 B of codes and 16 B per
+// 256-element block of absmax: 26 B + 1/16 B per parameter with clipping.
 //
 // The trainable set is described by a CHUNK TABLE (int64 pairs: offset, length; offsets and lengths are multiples of 64
 // elements, a chunk never straddles the matrix/vector boundary of the arena): one launch covers every parameter of a
@@ -42,6 +44,53 @@ __device__ __forceinline__ void adamw_one(float& p, float g, float& m, float& v,
     p -= (a.lr / a.bias_c1) * (m / denom);
 }
 
+__device__ __forceinline__ AdamWArgs load_hp(const float* hp) {
+    AdamWArgs a;
+    a.lr = hp[0]; a.beta1 = hp[1]; a.beta2 = hp[2]; a.eps = hp[3]; a.weight_decay = hp[4];
+    a.bias_c1 = hp[5]; a.bias_c2_sqrt = hp[6]; a.grad_scale = hp[7];
+    return a;
+}
+
+// One chunk with fp32 state, the block's threads striding over it: elements [off, off + len) of p, g, shadow (written when sh)
+// and g16 (may be NULL), state elements [soff, soff + len) of m and v.
+__device__ __forceinline__ void adamw_chunk_f32(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
+                                                __nv_bfloat16* __restrict__ shadow, bool sh, const __nv_bfloat16* __restrict__ g16,
+                                                int64_t off, int64_t soff, int64_t len, const AdamWArgs& a, int zero_grad) {
+    float4* p4 = reinterpret_cast<float4*>(p + off);
+    float4* g4 = reinterpret_cast<float4*>(g + off);
+    float4* m4 = reinterpret_cast<float4*>(m + soff);
+    float4* v4 = reinterpret_cast<float4*>(v + soff);
+    uint2* s2 = reinterpret_cast<uint2*>(shadow + off);
+    const uint2* h2 = reinterpret_cast<const uint2*>(g16 + off);
+    const int nv = int(len >> 2);
+    for (int i = threadIdx.x; i < nv; i += blockDim.x) {
+        float4 pp = p4[i];
+        float4 gg;
+        if (g16) {
+            const uint2 h = __ldg(h2 + i);
+            gg = make_float4(bf16_lo(h.x), bf16_hi(h.x), bf16_lo(h.y), bf16_hi(h.y));
+        } else {
+            gg = g4[i];
+        }
+        float4 mm = m4[i];
+        float4 vv = v4[i];
+        adamw_one(pp.x, gg.x, mm.x, vv.x, a);
+        adamw_one(pp.y, gg.y, mm.y, vv.y, a);
+        adamw_one(pp.z, gg.z, mm.z, vv.z, a);
+        adamw_one(pp.w, gg.w, mm.w, vv.w, a);
+        p4[i] = pp;
+        m4[i] = mm;
+        v4[i] = vv;
+        if (sh) {
+            uint2 q;
+            q.x = pack_bf16(pp.x, pp.y);
+            q.y = pack_bf16(pp.z, pp.w);
+            s2[i] = q;
+        }
+        if (zero_grad) g4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+}
+
 // g16 != NULL: the gradient comes from the bf16 communication buffer (the all-reduced, averaged gradient of a data-parallel
 // step); the fp32 accumulation buffer g is then only zeroed.
 __global__ void __launch_bounds__(256) adamw_chunks_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m,
@@ -49,44 +98,134 @@ __global__ void __launch_bounds__(256) adamw_chunks_kernel(float* __restrict__ p
                                                            const int64_t* __restrict__ chunks, int n_chunks, const float* __restrict__ hp,
                                                            int zero_grad, const __nv_bfloat16* __restrict__ g16) {
     pdl_sync();
-    AdamWArgs a;
-    a.lr = hp[0]; a.beta1 = hp[1]; a.beta2 = hp[2]; a.eps = hp[3]; a.weight_decay = hp[4];
-    a.bias_c1 = hp[5]; a.bias_c2_sqrt = hp[6]; a.grad_scale = hp[7];
+    const AdamWArgs a = load_hp(hp);
     for (int c = blockIdx.x; c < n_chunks; c += gridDim.x) {
         const int64_t off = chunks[2 * c], len = chunks[2 * c + 1];
         const bool sh = shadow != nullptr && off < n_shadow;
-        float4* p4 = reinterpret_cast<float4*>(p + off);
-        float4* g4 = reinterpret_cast<float4*>(g + off);
-        float4* m4 = reinterpret_cast<float4*>(m + off);
-        float4* v4 = reinterpret_cast<float4*>(v + off);
-        uint2* s2 = reinterpret_cast<uint2*>(shadow + off);
-        const uint2* h2 = reinterpret_cast<const uint2*>(g16 + off);
-        const int nv = int(len >> 2);
-        for (int i = threadIdx.x; i < nv; i += blockDim.x) {
-            float4 pp = p4[i];
-            float4 gg;
-            if (g16) {
-                const uint2 h = __ldg(h2 + i);
-                gg = make_float4(bf16_lo(h.x), bf16_hi(h.x), bf16_lo(h.y), bf16_hi(h.y));
-            } else {
-                gg = g4[i];
+        adamw_chunk_f32(p, g, m, v, shadow, sh, g16, off, off, len, a, zero_grad);
+    }
+}
+
+// Blockwise 8-bit AdamW (optim.AdamW8bit; Dettmers et al., ICLR 2022).  Chunk rows are int64 quadruples (arena offset, length,
+// state offset, bits).  bits == 32: fp32 m32 / v32 at the state offset, exactly adamw_chunks' update.  bits == 8: the row's
+// 256-element blocks (the last one may hold 64, 128 or 192) each keep one uint8 code per element and one fp32 absmax per
+// moment; m uses the signed map qmaps[0..255], v the unsigned map qmaps[256..511].  Per block (one warp, 8 elements per lane):
+// dequantise (map[code] * absmax), adamw_one on the unquantised moments, new absmax = block max |m| (|v|), new code = nearest
+// map entry: the smallest i with x <= 0.5f * (map[i] + map[i+1]).  A block whose absmax is 0 stores the code of 0.0.
+// The 255 midpoints are searched as an implicit (Eytzinger) binary tree in shared memory: level d of the tree is 2^d
+// consecutive floats, so the lanes of a warp hit distinct banks on the first six of the eight levels.
+constexpr int kQBlock = 256;
+
+__device__ __forceinline__ uint32_t quantize(float x, float absmax, const float* tree, uint32_t zero_code) {
+    if (absmax == 0.f) return zero_code;
+    x = x / absmax;
+    uint32_t k = 1;
+#pragma unroll
+    for (int l = 0; l < 8; ++l) k = 2 * k + (x > tree[k] ? 1u : 0u);
+    return k - 256;
+}
+
+__global__ void __launch_bounds__(256) adamw8bit_chunks_kernel(float* __restrict__ p, float* __restrict__ g, __nv_bfloat16* __restrict__ shadow,
+                                                               int64_t n_shadow, const int64_t* __restrict__ chunks, int n_chunks,
+                                                               const float* __restrict__ hp, const float* __restrict__ qmaps, float* __restrict__ m32,
+                                                               float* __restrict__ v32, uint8_t* __restrict__ qm, uint8_t* __restrict__ qv,
+                                                               float* __restrict__ absmax_m, float* __restrict__ absmax_v, int zero_grad,
+                                                               const __nv_bfloat16* __restrict__ g16) {
+    __shared__ float map_m[256], map_v[256], tree_m[256], tree_v[256];
+    __shared__ uint32_t zero_m;
+    pdl_sync();
+    const int t = threadIdx.x;
+    map_m[t] = qmaps[t];
+    map_v[t] = qmaps[256 + t];
+    __syncthreads();
+    if (t > 0) {   // tree node t at depth d holds the midpoint of in-order rank ((2 (t - 2^d) + 1) << (7 - d)) - 1
+        const int d = 31 - __clz(t);
+        const int i = ((2 * (t - (1 << d)) + 1) << (7 - d)) - 1;
+        tree_m[t] = 0.5f * (map_m[i] + map_m[i + 1]);
+        tree_v[t] = 0.5f * (map_v[i] + map_v[i + 1]);
+    }
+    if (map_m[t] == 0.f) zero_m = uint32_t(t);
+    __syncthreads();
+    const uint32_t zm = zero_m, zv = 0;   // the unsigned map starts at 0.0
+    const AdamWArgs a = load_hp(hp);
+    const int lane = t & 31, warp = t >> 5;
+    for (int c = blockIdx.x; c < n_chunks; c += gridDim.x) {
+        const int64_t off = chunks[4 * c], len = chunks[4 * c + 1], soff = chunks[4 * c + 2];
+        const bool sh = shadow != nullptr && off < n_shadow;
+        if (chunks[4 * c + 3] != 8) {   // uniform across the thread block
+            adamw_chunk_f32(p, g, m32, v32, shadow, sh, g16, off, soff, len, a, zero_grad);
+            continue;
+        }
+        const int nblk = int((len + kQBlock - 1) / kQBlock);
+        for (int b = warp; b < nblk; b += blockDim.x >> 5) {
+            const int64_t e0 = int64_t(b) * kQBlock;          // element of the row where this block starts
+            const int nb = int(min(int64_t(kQBlock), len - e0));  // 64, 128, 192 or 256
+            const int64_t qb = soff / kQBlock + b;             // block index into absmax
+            const float am_old = absmax_m[qb], av_old = absmax_v[qb];
+            float pe[8], me[8], ve[8];
+            bool ok[2];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {   // lane owns elements h*128 + 4*lane .. +3 of the block: two 16-byte loads
+                const int j = h * 128 + 4 * lane;
+                ok[h] = j < nb;
+                if (!ok[h]) {
+#pragma unroll
+                    for (int u = 0; u < 4; ++u) pe[4 * h + u] = me[4 * h + u] = ve[4 * h + u] = 0.f;
+                    continue;
+                }
+                const int64_t e = off + e0 + j;
+                const float4 pp = *reinterpret_cast<const float4*>(p + e);
+                float4 gg;
+                if (g16) {
+                    const uint2 hh = __ldg(reinterpret_cast<const uint2*>(g16 + e));
+                    gg = make_float4(bf16_lo(hh.x), bf16_hi(hh.x), bf16_lo(hh.y), bf16_hi(hh.y));
+                } else {
+                    gg = *reinterpret_cast<const float4*>(g + e);
+                }
+                const uint32_t cm = *reinterpret_cast<const uint32_t*>(qm + soff + e0 + j);
+                const uint32_t cv = *reinterpret_cast<const uint32_t*>(qv + soff + e0 + j);
+                const float gl[4] = {gg.x, gg.y, gg.z, gg.w};
+                pe[4 * h] = pp.x; pe[4 * h + 1] = pp.y; pe[4 * h + 2] = pp.z; pe[4 * h + 3] = pp.w;
+#pragma unroll
+                for (int u = 0; u < 4; ++u) {
+                    float& m = me[4 * h + u];
+                    float& v = ve[4 * h + u];
+                    m = map_m[(cm >> (8 * u)) & 0xFF] * am_old;
+                    v = map_v[(cv >> (8 * u)) & 0xFF] * av_old;
+                    adamw_one(pe[4 * h + u], gl[u], m, v, a);
+                }
             }
-            float4 mm = m4[i];
-            float4 vv = v4[i];
-            adamw_one(pp.x, gg.x, mm.x, vv.x, a);
-            adamw_one(pp.y, gg.y, mm.y, vv.y, a);
-            adamw_one(pp.z, gg.z, mm.z, vv.z, a);
-            adamw_one(pp.w, gg.w, mm.w, vv.w, a);
-            p4[i] = pp;
-            m4[i] = mm;
-            v4[i] = vv;
-            if (sh) {
-                uint2 q;
-                q.x = pack_bf16(pp.x, pp.y);
-                q.y = pack_bf16(pp.z, pp.w);
-                s2[i] = q;
+            uint32_t mx_m = 0, mx_v = 0;   // |x| of finite floats orders like its bit pattern
+#pragma unroll
+            for (int u = 0; u < 8; ++u) {
+                mx_m = max(mx_m, __float_as_uint(fabsf(me[u])));
+                mx_v = max(mx_v, __float_as_uint(fabsf(ve[u])));
             }
-            if (zero_grad) g4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+            const float am = __uint_as_float(__reduce_max_sync(0xffffffffu, mx_m));
+            const float av = __uint_as_float(__reduce_max_sync(0xffffffffu, mx_v));
+            if (lane == 0) {
+                absmax_m[qb] = am;
+                absmax_v[qb] = av;
+            }
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                if (!ok[h]) continue;
+                const int j = h * 128 + 4 * lane;
+                const int64_t e = off + e0 + j;
+                uint32_t cm = 0, cv = 0;
+#pragma unroll
+                for (int u = 0; u < 4; ++u) {
+                    cm |= quantize(me[4 * h + u], am, tree_m, zm) << (8 * u);
+                    cv |= quantize(ve[4 * h + u], av, tree_v, zv) << (8 * u);
+                }
+                *reinterpret_cast<uint32_t*>(qm + soff + e0 + j) = cm;
+                *reinterpret_cast<uint32_t*>(qv + soff + e0 + j) = cv;
+                *reinterpret_cast<float4*>(p + e) = make_float4(pe[4 * h], pe[4 * h + 1], pe[4 * h + 2], pe[4 * h + 3]);
+                if (sh)
+                    *reinterpret_cast<uint2*>(shadow + e) =
+                        make_uint2(pack_bf16(pe[4 * h], pe[4 * h + 1]), pack_bf16(pe[4 * h + 2], pe[4 * h + 3]));
+                if (zero_grad) *reinterpret_cast<float4*>(g + e) = make_float4(0.f, 0.f, 0.f, 0.f);
+            }
         }
     }
 }
@@ -186,6 +325,23 @@ int t2v_adamw_chunks(float* p, float* g, const void* g_bf16, float* m, float* v,
                                   v, static_cast<__nv_bfloat16*>(shadow_bf16), n_shadow, chunks, int(n_chunks), hp, int(zero_grad),
                                   static_cast<const __nv_bfloat16*>(g_bf16)));
     return launch_checked(rc, "adamw_chunks");
+}
+
+int t2v_adamw8bit_chunks(float* p, float* g, const void* g_bf16, void* shadow_bf16, int64_t n_shadow, const int64_t* chunks, int32_t n_chunks,
+                         const float* hp, const float* qmaps, float* m32, float* v32, void* code_m, void* code_v, float* absmax_m,
+                         float* absmax_v, int32_t zero_grad, void* stream) {
+    if (n_chunks <= 0) return 0;
+    if ((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(m32) | reinterpret_cast<uintptr_t>(v32)) &
+        15u)
+        return fail(-2, "adamw8bit_chunks: p, g, m32, v32 must be 16-byte aligned");
+    if ((reinterpret_cast<uintptr_t>(code_m) | reinterpret_cast<uintptr_t>(code_v)) & 3u)
+        return fail(-2, "adamw8bit_chunks: code_m, code_v must be 4-byte aligned");
+    if (shadow_bf16 && (reinterpret_cast<uintptr_t>(shadow_bf16) & 7u)) return fail(-2, "adamw8bit_chunks: shadow must be 8-byte aligned");
+    const int rc = int(launch_pdl(adamw8bit_chunks_kernel, dim3(chunk_grid(n_chunks)), dim3(256), size_t(0), static_cast<cudaStream_t>(stream), p,
+                                  g, static_cast<__nv_bfloat16*>(shadow_bf16), n_shadow, chunks, int(n_chunks), hp, qmaps, m32, v32,
+                                  static_cast<uint8_t*>(code_m), static_cast<uint8_t*>(code_v), absmax_m, absmax_v, int(zero_grad),
+                                  static_cast<const __nv_bfloat16*>(g_bf16)));
+    return launch_checked(rc, "adamw8bit_chunks");
 }
 
 int t2v_counter_add(int64_t* counter, int64_t value, void* stream) {

@@ -8,6 +8,9 @@ gradient ranges it consumed (no per-step memset).  Nothing in `launch()` touches
 into the CUDA graph of the training step; the learning rate reaches the device through `push_hyperparams()`.
 
 Frozen parameters are never touched (torch semantics: grad None => skipped, no weight decay either).
+
+`AdamW8bit` (`use_8bit_adam`, reference train.py:238-249) is the same step with blockwise 8-bit moments for tensors of at
+least 4096 elements; its algorithm is stated on the class and on `dynamic_map`.
 """
 import torch
 
@@ -23,8 +26,6 @@ class FusedAdamW(torch.optim.Optimizer):
         self.arena = arena
         self.max_grad_norm = max_grad_norm
         dev = arena.master.device
-        self.exp_avg = torch.zeros_like(arena.master)
-        self.exp_avg_sq = torch.zeros_like(arena.master)
         self.state_dev = torch.zeros(1, device=dev, dtype=torch.int64)     # [0] optimizer step count
         self.sq = torch.zeros(2, device=dev, dtype=torch.float64)          # [0] sum g^2 (running), [1] last gradient norm
         self._off = {id(p): o for p, o in zip(arena.params, arena.offsets)}
@@ -32,8 +33,21 @@ class FusedAdamW(torch.optim.Optimizer):
             for p in group["params"]:
                 if id(p) not in self._off:
                     raise ValueError("FusedAdamW only drives parameters that live in the arena")
+        self._alloc_state()
         self._sets = None
         self._build()
+
+    def _alloc_state(self):
+        self.exp_avg = torch.zeros_like(self.arena.master)
+        self.exp_avg_sq = torch.zeros_like(self.arena.master)
+
+    def _moments(self):
+        """Name -> device tensor of the optimizer's moment state (what `state_dict` saves besides the step count)."""
+        return {"exp_avg": self.exp_avg, "exp_avg_sq": self.exp_avg_sq}
+
+    def state_tensors(self):
+        """Every device tensor one step mutates besides the weights and gradients (a CUDA-graph capture snapshots them)."""
+        return list(self._moments().values()) + [self.state_dev, self.sq]
 
     # ------------------------------------------------------------------------------------------------ chunk tables
     @staticmethod
@@ -52,28 +66,34 @@ class FusedAdamW(torch.optim.Optimizer):
                 runs.append([a, b])
         return runs
 
+    def _table(self, params):
+        """Update-kernel rows (offset, length) over the trainable `params`, never straddling the matrix / vector boundary."""
+        n_mat = self.arena.n_mat
+        chunks = []
+        for a, b in self._runs(params):
+            for lo, hi in ((a, min(b, n_mat)), (max(a, n_mat), b)):
+                pos = lo
+                while pos < hi:
+                    n = min(CHUNK, hi - pos)
+                    chunks.append((pos, n))
+                    pos += n
+        return chunks
+
     def _build(self):
         """Groups with identical hyper-parameters form one set: one chunk table, one row of device hyper-parameters."""
         by_key = {}
         for gi, group in enumerate(self.param_groups):
             by_key.setdefault(self._key(group), []).append(gi)
         dev = self.arena.master.device
-        n_mat = self.arena.n_mat
         sets = []
         for key, gis in by_key.items():
             params = [p for gi in gis for p in self.param_groups[gi]["params"]]
-            chunks = []
-            for a, b in self._runs(params):
-                for lo, hi in ((a, min(b, n_mat)), (max(a, n_mat), b)):     # never straddle the matrix / vector boundary
-                    pos = lo
-                    while pos < hi:
-                        n = min(CHUNK, hi - pos)
-                        chunks.append((pos, n))
-                        pos += n
+            chunks = self._table(params)
             if not chunks:
                 continue
-            sets.append({"groups": gis, "key": key, "chunks": torch.tensor(chunks, dtype=torch.int64, device=dev).contiguous(),
-                         "n": sum(n for _, n in chunks)})
+            table = torch.tensor(chunks, dtype=torch.int64, device=dev).contiguous()
+            sets.append({"groups": gis, "key": key, "chunks": table, "norm_chunks": table[:, :2].contiguous() if table.shape[1] > 2 else table,
+                         "n": sum(c[1] for c in chunks)})
         if not sets:
             raise ValueError("FusedAdamW: no trainable parameters")
         self._sets = sets
@@ -115,11 +135,14 @@ class FusedAdamW(torch.optim.Optimizer):
         ar = self.arena
         if self.max_grad_norm is not None:
             for s in self._sets:
-                prims.sqnorm_chunks(ar.grad, s["chunks"], self.sq, grad_bf16)
+                prims.sqnorm_chunks(ar.grad, s["norm_chunks"], self.sq, grad_bf16)
         prims.adamw_prepare(self.hp_in, self.hp, self.state_dev, self.sq, self.max_grad_norm or 0.0)
         for i, s in enumerate(self._sets):
-            prims.adamw_chunks(ar.master, ar.grad, self.exp_avg, self.exp_avg_sq, ar.shadow, ar.n_mat, s["chunks"], self.hp[i], zero_grad,
-                               grad_bf16)
+            self._update(s, self.hp[i], zero_grad, grad_bf16)
+
+    def _update(self, s, hp_row, zero_grad, grad_bf16):
+        ar = self.arena
+        prims.adamw_chunks(ar.master, ar.grad, self.exp_avg, self.exp_avg_sq, ar.shadow, ar.n_mat, s["chunks"], hp_row, zero_grad, grad_bf16)
 
     @torch.no_grad()
     def step(self, closure=None, zero_grad=True):
@@ -143,13 +166,99 @@ class FusedAdamW(torch.optim.Optimizer):
     # ------------------------------------------------------------------------------------------------ checkpointing
     def state_dict(self):
         d = super().state_dict()
-        d["fused"] = {"exp_avg": self.exp_avg, "exp_avg_sq": self.exp_avg_sq, "step": self.steps}
+        d["fused"] = dict(self._moments(), step=self.steps)
         return d
 
     def load_state_dict(self, state_dict):
         fused = state_dict.pop("fused", None)
         super().load_state_dict(state_dict)
         if fused is not None:
-            self.exp_avg.copy_(fused["exp_avg"])
-            self.exp_avg_sq.copy_(fused["exp_avg_sq"])
+            for name, t in self._moments().items():
+                t.copy_(fused[name])
             self.state_dev.fill_(int(fused["step"]))
+
+
+# ---------------------------------------------------------------------------------------------------- blockwise 8-bit AdamW
+MIN_8BIT_SIZE = 4096   # tensors with fewer elements keep fp32 moments
+QBLOCK = 256           # elements per quantisation block
+
+
+def dynamic_map(signed):
+    """The 256-entry dynamic-tree quantisation map of Dettmers et al., *8-bit Optimizers via Block-wise Quantization*
+    (ICLR 2022), with bitsandbytes' `create_dynamic_map` defaults (7 exponent levels, 8 bits), as sorted fp32 values.
+
+    A code's leading zero bits select a decade 10^(e-6), e = 0..6; the bits after the first one (the indicator) select one
+    of 2^k linearly spaced fractions of that decade: the midpoints of `linspace(0.1, 1, 2^k + 1)`.  Signed (for m): one
+    sign bit, so decade e holds 2^e fractions, each with both signs (2 * 127 values).  Unsigned (for v): decade e holds
+    2^(e+1) fractions (254 values).  0 and 1 are added, so both maps hold 256 distinct entries, contain 0 and 1 exactly, and
+    are densest near 0, where most normalised moments fall.  Computed in fp32 like the reference construction."""
+    data = []
+    for e in range(7):
+        n = 2 ** e if signed else 2 ** (e + 1)
+        bounds = torch.linspace(0.1, 1, n + 1, dtype=torch.float32)
+        means = (bounds[:-1] + bounds[1:]) / 2.0
+        data += ((10 ** (e - 6)) * means).tolist()
+        if signed:
+            data += (-(10 ** (e - 6)) * means).tolist()
+    data += [0.0, 1.0]
+    assert len(data) == 256
+    return torch.tensor(sorted(data), dtype=torch.float32)
+
+
+class AdamW8bit(FusedAdamW):
+    """AdamW with blockwise 8-bit moments (bitsandbytes `AdamW8bit` defaults: block size 256, `min_8bit_size` 4096, no
+    percentile clipping) on the flat arena; the reference builds `bitsandbytes.optim.AdamW8bit` for `use_8bit_adam`.
+
+    A trainable tensor with fewer than MIN_8BIT_SIZE elements keeps fp32 m and v and gets exactly FusedAdamW's update.  A
+    larger one is cut into blocks of QBLOCK consecutive elements from its first element; each block stores one uint8 code
+    per element and one fp32 absmax per moment, m through the signed `dynamic_map`, v through the unsigned one.  Per element:
+        g *= clip;  m = b1 * deq(m) + (1 - b1) * g;  v = b2 * deq(v) + (1 - b2) * g^2   with deq(c) = map[c] * absmax_old
+        p *= 1 - lr * wd;  p -= (lr / bc1) * m / (sqrt(v) / sqrt(bc2) + eps)          (the unquantised fp32 m and v)
+    then per block absmax = max |m| (|v|) and code = the smallest i with m / absmax <= 0.5f * (map[i] + map[i+1]); a block
+    whose absmax is 0 stores the code of 0.0.  The state is compact: it covers the trainable tensors only, in arena order,
+    each tensor's 8-bit state starting at a multiple of QBLOCK.  One update launch per hyper-parameter set
+    (csrc/optim.cu adamw8bit_chunks_kernel); the clipping norm and the device scalars are FusedAdamW's."""
+
+    def _alloc_state(self):
+        dev = self.arena.master.device
+        self._layout, n8, n32 = {}, 0, 0   # id(param) -> (bits, state offset)
+        params = [p for g in self.param_groups for p in g["params"] if p.requires_grad]
+        for p in sorted(params, key=lambda q: self._off[id(q)]):
+            n = _align(p.numel())
+            if p.numel() >= MIN_8BIT_SIZE:
+                self._layout[id(p)] = (8, n8)
+                n8 += _align(n, QBLOCK)
+            else:
+                self._layout[id(p)] = (32, n32)
+                n32 += n
+        self.qmaps = torch.cat([dynamic_map(True), dynamic_map(False)]).to(dev)
+        zero_m = int((self.qmaps[:256] == 0).nonzero()[0, 0])
+        self.code_m = torch.full((n8,), zero_m, device=dev, dtype=torch.uint8)
+        self.code_v = torch.zeros(n8, device=dev, dtype=torch.uint8)   # the unsigned map starts at 0.0
+        self.absmax_m = torch.zeros(n8 // QBLOCK, device=dev, dtype=torch.float32)
+        self.absmax_v = torch.zeros(n8 // QBLOCK, device=dev, dtype=torch.float32)
+        self.exp_avg32 = torch.zeros(n32, device=dev, dtype=torch.float32)
+        self.exp_avg_sq32 = torch.zeros(n32, device=dev, dtype=torch.float32)
+
+    def _moments(self):
+        return {"code_m": self.code_m, "code_v": self.code_v, "absmax_m": self.absmax_m, "absmax_v": self.absmax_v,
+                "exp_avg32": self.exp_avg32, "exp_avg_sq32": self.exp_avg_sq32}
+
+    def state_bytes(self):
+        return sum(t.numel() * t.element_size() for t in self._moments().values())
+
+    def _table(self, params):
+        """Rows (arena offset, length, state offset, bits): at most CHUNK elements, inside one tensor (CHUNK is a multiple of
+        QBLOCK, so every 8-bit row but a tensor's last covers whole blocks)."""
+        rows = []
+        for p in sorted((p for p in params if p.requires_grad), key=lambda q: self._off[id(q)]):
+            a, n = self._off[id(p)], _align(p.numel())
+            bits, s = self._layout[id(p)]
+            for lo in range(0, n, CHUNK):
+                rows.append((a + lo, min(CHUNK, n - lo), s + lo, bits))
+        return rows
+
+    def _update(self, s, hp_row, zero_grad, grad_bf16):
+        ar = self.arena
+        prims.adamw8bit_chunks(ar.master, ar.grad, ar.shadow, ar.n_mat, s["chunks"], hp_row, self.qmaps, self.exp_avg32, self.exp_avg_sq32,
+                               self.code_m, self.code_v, self.absmax_m, self.absmax_v, zero_grad, grad_bf16)

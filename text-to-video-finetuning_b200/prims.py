@@ -349,6 +349,19 @@ def adamw_chunks(p, g, m, v, shadow, n_shadow, chunks, hp_row, zero_grad=True, g
                                                _p(hp_row), int(bool(zero_grad)), _stream()))
 
 
+def adamw8bit_chunks(p, g, shadow, n_shadow, chunks, hp_row, qmaps, m32, v32, code_m, code_v, absmax_m, absmax_v, zero_grad=True,
+                     g_bf16=None):
+    """Blockwise 8-bit AdamW over the (arena offset, length, state offset, bits) rows of one hyper-parameter set: fp32 m32 / v32
+    for 32-bit rows, uint8 codes into qmaps (512 floats: signed map, unsigned map) times per-256-block absmax for 8-bit rows."""
+    _chk_f32(p, g, hp_row, qmaps, m32, v32, absmax_m, absmax_v)
+    _chk_bf16(shadow, g_bf16)
+    assert chunks.dtype == torch.int64 and chunks.dim() == 2 and chunks.shape[1] == 4 and chunks.is_contiguous()
+    assert code_m.dtype == code_v.dtype == torch.uint8 and code_m.is_cuda and code_v.is_cuda and qmaps.numel() == 512
+    native.check(native.lib().t2v_adamw8bit_chunks(_p(p), _p(g), _p(g_bf16), _p(shadow), int(n_shadow), _p(chunks), chunks.shape[0],
+                                                   _p(hp_row), _p(qmaps), _p(m32), _p(v32), _p(code_m), _p(code_v), _p(absmax_m),
+                                                   _p(absmax_v), int(bool(zero_grad)), _stream()))
+
+
 def scale_cast_f32_bf16(src, dst, alpha):
     """dst (bf16) = alpha * src (fp32): gradient compression before the data-parallel all-reduce."""
     _chk_f32(src)

@@ -144,7 +144,7 @@ class DataParallelStep:
             keep += [self.arena.master, self.arena.grad, self.arena.shadow]
         opt = self.optimizer
         if opt is not None and hasattr(opt, "launch"):
-            keep += [opt.exp_avg, opt.exp_avg_sq, opt.state_dev, opt.sq]
+            keep += opt.state_tensors()
         keep.append(ops.dropout_epoch(self.abar.device))
         return keep
 

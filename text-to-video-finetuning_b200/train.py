@@ -244,8 +244,9 @@ def main(
         dist.init_process_group("nccl", device_id=dev)
     if train_text_encoder or use_text_lora:
         raise NotImplementedError("text-encoder training is outside the H100 hot path of this build (SURVEY 8(f) row 2)")
-    if use_8bit_adam:
-        raise NotImplementedError("bitsandbytes 8-bit Adam is not available; fused AdamW is SURVEY 8(f) row 1")
+    fused_adamw = bool(kwargs.get("fused_adamw", True))   # optim.FusedAdamW on the flat arena (SURVEY 8(f) row 1); False: torch AdamW
+    if use_8bit_adam and not fused_adamw:
+        raise ValueError("use_8bit_adam runs optim.AdamW8bit on the flat arena; it cannot be combined with fused_adamw=False")
     if seed is not None:
         # model construction and LoRA initialisation (lora_down ~ N(0, 1/r)) must be identical on every rank: the reference
         # gets that from accelerate/DDP broadcasting rank 0's parameters at wrap time (train.py:661).  The per-rank stream
@@ -287,11 +288,11 @@ def main(
         stepper.arena.refresh_shadow()
     if seed is not None:
         torch.manual_seed(seed + rank)
-    fused_adamw = bool(kwargs.get("fused_adamw", True))   # optim.FusedAdamW on the flat arena (SURVEY 8(f) row 1); False: torch AdamW
     if fused_adamw:
-        from .optim import FusedAdamW
-        optimizer = FusedAdamW(stepper.arena, groups, lr=learning_rate, betas=(adam_beta1, adam_beta2), weight_decay=adam_weight_decay,
-                               eps=adam_epsilon, max_grad_norm=max_grad_norm)
+        from .optim import AdamW8bit, FusedAdamW
+        cls = AdamW8bit if use_8bit_adam else FusedAdamW
+        optimizer = cls(stepper.arena, groups, lr=learning_rate, betas=(adam_beta1, adam_beta2), weight_decay=adam_weight_decay,
+                        eps=adam_epsilon, max_grad_norm=max_grad_norm)
         stepper.attach_optimizer(optimizer)   # the update (clip + AdamW + shadow refresh + grad zeroing) is part of the step graph
     else:
         optimizer = torch.optim.AdamW(groups, lr=learning_rate, betas=(adam_beta1, adam_beta2), weight_decay=adam_weight_decay,
