@@ -61,6 +61,13 @@ Overrides read_overrides() {
 
 int b_stage_bytes(int bn, bool b_mn) { return b_mn ? ((bn + 63) / 64) * 8192 : bn * 128; }
 
+// Shared memory the pipeline stages of an N = bn launch may use.  It still holds back the 16.5 KB of staging the epilogue
+// needed before it moved into its own warpgroup of four warps: handing that space to the stages would change the stage
+// count of most launches, a planner decision that tests/golden/gemm_plans.json pins and that a sweep of its own
+// (tools/plan_sweep.py) has to justify.
+constexpr int kStageBudgetHoldback = 4 * 4096 + 4 * 128;
+int stage_budget(int bn, int smem_reserve) { return kMaxSmemBytes - gemm_fixed_smem_bytes(bn) - kStageBudgetHoldback - smem_reserve; }
+
 // A (wgmma N, split-K factor) candidate as the cost models see it.
 struct Cand {
     int bn, s, kper;       // N, split factor, k-blocks per split
@@ -81,7 +88,7 @@ Cand search(int64_t row_tiles, int ncols, bool b_mn, int kblocks, int smem_reser
         if (forced_bn && bn != forced_bn) continue;
         if (bn > 16 && bn - 16 >= ncols) continue;
         const int stage_bytes = kBlockM * 128 + b_stage_bytes(bn, b_mn);
-        if ((kMaxSmemBytes - gemm_fixed_smem_bytes(bn) - smem_reserve) / stage_bytes < 3) continue;
+        if (stage_budget(bn, smem_reserve) / stage_bytes < 3) continue;
         const int64_t base = row_tiles * ((ncols + bn - 1) / bn);
         const int max_s = max_split(base);
         for (int s = 1; s <= max_s; ++s) {
@@ -131,7 +138,7 @@ double acc_split_cost(const Cand& c) { return double(c.waves) * (c.kper * kAccKB
 void finish_common(GemmParams& p, bool b_mn, int forced_stages, int smem_reserve) {
     p.stage_bytes_a = kBlockM * 128;
     p.stage_bytes_b = b_stage_bytes(p.block_n, b_mn);
-    const int budget = kMaxSmemBytes - gemm_fixed_smem_bytes(p.block_n) - smem_reserve;
+    const int budget = stage_budget(p.block_n, smem_reserve);
     p.num_stages = std::min<int>(kMaxStages, budget / (p.stage_bytes_a + p.stage_bytes_b));
     if (forced_stages) p.num_stages = std::min(p.num_stages, forced_stages);
     int64_t tiles = 1;

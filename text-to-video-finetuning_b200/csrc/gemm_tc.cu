@@ -1,12 +1,14 @@
 // Persistent warp-specialised wgmma GEMM for sm_90a.  See gemm_tc.cuh for the operand model.
 //
-//   warp 8    : TMA producer (one elected lane of warpgroup 2) - fills the smem ring, one mbarrier pair per stage
-//   warps 0-7 : two consumer warpgroups.  Warpgroup g runs wgmma on rows 64g..64g+63 of the 128-row tile (fp32 accumulator
-//               in registers), then stores the accumulator to shared memory and runs the fused epilogue on the same rows:
-//               thread <-> output row, the two warp pairs of a warpgroup split the columns; smem-staged coalesced global
-//               stores / red.add.
+//   warps 0-7   : two MMA warpgroups.  Warpgroup g runs wgmma on rows 64g..64g+63 of the 128-row tile (fp32 accumulator in
+//                 registers), then hands the finished accumulator to the epilogue through shared memory.
+//   warp 8      : TMA producer (one elected lane of warpgroup 2) - fills the smem ring, one mbarrier pair per stage
+//   warps 12-15 : the epilogue warpgroup.  Thread <-> output row (warp w owns rows 32w..32w+31 and every column chunk);
+//                 smem-staged coalesced global stores / red.add.
 //
-// The producer keeps filling the ring during the epilogue, so the next tile's main loop starts on loaded stages.
+// The accumulator tile in shared memory is handed over with two mbarriers: acc_full (MMA -> epilogue) and acc_empty
+// (epilogue -> MMA, arrived once the epilogue has read the last accumulator chunk, before that chunk's global stores).  So
+// the MMA warpgroups start the next tile's main loop while the epilogue of the previous one is still running.
 #include "common.h"
 #include "gemm_tc.cuh"
 #include "ptx.cuh"
@@ -37,7 +39,8 @@ __device__ __forceinline__ void k_range(const GemmParams& p, const TileVars& tv,
     if (p.ksplit_var >= 0) {
         int32_t sv = 0;
 #pragma unroll
-        for (int i = 0; i < 6; ++i) sv = (i == p.ksplit_var) ? tv.t[i] : sv;
+        for (int i = 0; i < 6; ++i) sv |= tv.t[i] & -static_cast<int32_t>(i == p.ksplit_var);   // (a select chain would be
+                                                                                                 // lowered to an indexed local array)
         kb0 = sv * p.kb_per_split;
         kb1 = min(p.kb_total, kb0 + p.kb_per_split);
     } else {
@@ -89,20 +92,21 @@ struct RuntimeFlag {
     __device__ constexpr operator bool() const { return v; }
 };
 
-// Epilogue of one tile (warps 0..7).  Warp w owns accumulator rows 64*(w/4) + 32*(w%2)..+31, i.e. thread <-> output row, and
-// the two warp pairs of a warpgroup split the columns.  Output rows are strided in global memory, so every 32-column chunk
-// goes through a per-warp swizzled staging tile and is moved with 16 bytes per lane covering whole rows (full 64/128-byte
-// segments); the residual comes in the same way.  The per-column bias is fetched with one coalesced load per chunk and
-// broadcast through shared memory.  Buffers that are not 16-byte aligned (EPI_VEC clear) take a per-thread scalar path.
-// rowsum_tile: rs_s holds the row sums of operand A for this tile (EPI_ROWSUM_A).
+// Epilogue of one tile (epilogue warp w = 0..3).  Warp w owns accumulator rows 32w..32w+31, i.e. thread <-> output row, and
+// all of the tile's column chunks.  Output rows are strided in global memory, so every 32-column chunk goes through a per-warp
+// swizzled staging tile and is moved with 16 bytes per lane covering whole rows (full 64/128-byte segments); the residual
+// comes in the same way.  The per-column bias is fetched with one coalesced load per chunk and broadcast through shared
+// memory.  Buffers that are not 16-byte aligned (EPI_VEC clear) take a per-thread scalar path.
+// The accumulator tile is read after acc_full completes phase acc_phase; every thread arrives on acc_empty once it has read
+// its last accumulator chunk (and row sum).  rowsum_tile: rs_s holds the row sums of operand A for this tile (EPI_ROWSUM_A).
 template <int ESZ>
 __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const TileVars& tv, bool rowsum_tile, uint32_t warp, uint32_t lane,
-                                              uint32_t acc_s, uint32_t acc_pitch, const float* rs_s, uint8_t* stg_base) {
+                                              uint32_t acc_s, uint32_t acc_pitch, uint32_t rs_s, uint8_t* stg_base,
+                                              uint64_t* acc_full, uint64_t* acc_empty, uint32_t acc_phase) {
     constexpr int CPR = ESZ * 2;        // 16-byte chunks per 32-column row: 4 (bf16) or 8 (fp32)
     constexpr int EPC = 16 / ESZ;       // elements per 16-byte chunk
     constexpr int RPI = 32 / CPR;       // rows covered by one warp-wide 16-byte access
-    const uint32_t grp = (warp >> 1) & 1u;
-    const uint32_t row = (warp >> 2) * 64u + (warp & 1u) * 32u + lane;
+    const uint32_t row = warp * 32u + lane;
     const int32_t rw = static_cast<int32_t>(row) % p.bw;
     const int32_t rh = (static_cast<int32_t>(row) / p.bw) % p.bh;
     const int32_t rn = static_cast<int32_t>(row) / (p.bw * p.bh);
@@ -110,30 +114,27 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const TileVar
     const bool vec = p.flags & EPI_VEC;
     const bool has_stats = ESZ == 2 && (p.flags & EPI_STATS) && vec;
     const int32_t col0 = tv.t[0] * p.block_n;
-    // this warp pair's half of the tile's 32-column chunks, without the chunks past the output's last column
-    const int nchunks = (p.block_n + 31) >> 5;
-    const int c_begin = grp == 0 ? 0 : (nchunks + 1) >> 1;
-    const int c_end = min(grp == 0 ? (nchunks + 1) >> 1 : nchunks, (p.ncols - col0 + 31) >> 5);
+    // the tile's 32-column chunks, without the chunks past the output's last column
+    const int c_end = min((p.block_n + 31) >> 5, (p.ncols - col0 + 31) >> 5);
     const uint32_t stg_s = smem_u32(stg_base + warp * 4096u);                   // 32 rows x <= 128 B
-    float* sbias = reinterpret_cast<float*>(stg_base + 8 * 4096u) + warp * 32;  // 32 floats per warp
+    float* sbias = reinterpret_cast<float*>(stg_base + 4 * 4096u) + warp * 32;  // 32 floats per warp
     // swizzled byte offset of logical 16-byte chunk j of row r in a dense [32][n] chunk array
     auto phys = [](int r, int j, int n) { return (r * n + (j ^ (((r * n) >> 3) & (n - 1)))) * 16; };
     const int sr = lane / CPR, sj = lane % CPR;  // (row-in-group, chunk) this lane moves in the coalesced phases
-    // tile-invariant shared-memory addresses of the staging tile (hoisted: the chunk body is straight-line code)
-    uint32_t w_own[CPR];     // this lane's own row, 16-byte chunk j                     (write after the math)
-    uint32_t r_mov[CPR];     // the (row, chunk) this lane moves in the coalesced store   (read)
-    uint32_t w_res[4];       // residual staging: row (lane / 4) + 8 i, chunk lane % 4   (write, bf16 rows of 64 B)
-    uint32_t r_res[4];       // residual staging: own row, chunk j                       (read)
-#pragma unroll
-    for (int j = 0; j < CPR; ++j) {
-        w_own[j] = stg_s + phys(static_cast<int>(lane), j, CPR);
-        r_mov[j] = stg_s + phys(sr + RPI * j, sj, CPR);
-    }
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-        w_res[j] = stg_s + phys(static_cast<int>(lane >> 2) + 8 * j, static_cast<int>(lane & 3), 4);
-        r_res[j] = stg_s + phys(static_cast<int>(lane), j, 4);
-    }
+    // Tile-invariant shared-memory addresses of the staging tile.  stg_s is 256-byte aligned and a staged row is CPR (or 4)
+    // chunks, so each family of addresses is one base register and a compile-time XOR or offset: rows 512 bytes apart share
+    // the swizzle key (up to bit 2 with 8 chunks a row), and the chunk index sits in the bits a row base leaves clear.
+    const uint32_t w_own0 = stg_s + phys(static_cast<int>(lane), 0, CPR);
+    const uint32_t r_mov0 = stg_s + phys(sr, sj, CPR);
+    const uint32_t w_res0 = stg_s + phys(static_cast<int>(lane >> 2), static_cast<int>(lane & 3), 4);
+    const uint32_t r_res0 = stg_s + phys(static_cast<int>(lane), 0, 4);
+    // this lane's own row, 16-byte chunk j (write after the math)
+    auto w_own = [&](int j) { return w_own0 ^ (static_cast<uint32_t>(j) << 4); };
+    // the (row sr + RPI j, chunk sj) this lane moves in the coalesced store (read); with 8 chunks a row, odd j flips key bit 2
+    auto r_mov = [&](int j) { return (r_mov0 ^ (CPR == 8 ? static_cast<uint32_t>(j & 1) << 6 : 0u)) + 512u * j; };
+    // residual staging (bf16 rows of 64 B): write row (lane / 4) + 8 j, chunk lane % 4; read own row, chunk j
+    auto w_res = [&](int j) { return w_res0 + 512u * j; };
+    auto r_res = [&](int j) { return r_res0 ^ (static_cast<uint32_t>(j) << 4); };
     const bool alpha_one = p.alpha == 1.0f;
     const int32_t gw = tv.t[1] * p.bw + rw, gh = tv.t[2] * p.bh + rh, gn = tv.t[3] * p.bn + rn;
     const bool row_ok = (rn < p.bn) && gw < p.W && gh < p.H && gn < p.N;
@@ -186,9 +187,9 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const TileVar
     // The residual is prefetched only when every row is in bounds, and only for a full-width chunk: only a full chunk uses it
     const bool res_pref = all_rows && has_res;
     const __nv_bfloat16* res_lane = static_cast<const __nv_bfloat16*>(p.residual) + (lane & 3) * 8;
-    int64_t off_q[4];   // residual rows this lane fetches: (lane / 4) + 8 i
+    int64_t off_q[4];   // residual rows this lane fetches: (lane / 4) + 8 i - for bf16 output the rows of off_s
 #pragma unroll
-    for (int i = 0; i < 4; ++i) off_q[i] = __shfl_sync(0xffffffffu, off, (lane >> 2) + 8 * i);
+    for (int i = 0; i < 4; ++i) off_q[i] = ESZ == 2 ? off_s[i] : __shfl_sync(0xffffffffu, off, (lane >> 2) + 8 * i);
     auto load_res = [&](int ch, uint4 (&q)[4]) {
         const int32_t c = col0 + ch * 32;
         if (min(p.block_n - ch * 32, p.ncols - c) >= 32) {
@@ -198,13 +199,17 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const TileVar
     };
     float bq0 = 0.f, bq1 = 0.f;
     uint4 rq[4] = {};
-    if (c_begin < c_end) bq0 = load_colterm(c_begin);
-    if (c_begin + 1 < c_end) bq1 = load_colterm(c_begin + 1);
-    if (res_pref && c_begin < c_end) load_res(c_begin, rq);
+    if (c_end > 0) bq0 = load_colterm(0);
+    if (c_end > 1) bq1 = load_colterm(1);
+    if (res_pref && c_end > 0) load_res(0, rq);
+    mbar_wait(acc_full, acc_phase);
     const uint32_t arow = acc_s + row * acc_pitch * 4u, akey = acc_swz(row);
     uint32_t acc[32];
-    if (c_begin < c_end) acc_ld32(arow, akey, c_begin, acc);  // chunk ch+1 is read while chunk ch goes out to global memory
-    for (int ch = c_begin; ch < c_end; ++ch) {
+    if (c_end > 0) acc_ld32(arow, akey, 0, acc);  // chunk ch+1 is read while chunk ch goes out to global memory
+    // row sums of operand A (weight gradient: the bias gradient)
+    if (rowsum_tile && row_ok) atomicAdd(p.rowsum + gw, __uint_as_float(lds32(rs_s + row * 4u)));
+    if (c_end <= 1) mbar_arrive(acc_empty);   // (with more chunks: once the last one has been read, in its predecessor's body)
+    for (int ch = 0; ch < c_end; ++ch) {
         const int32_t col = col0 + ch * 32;
         const int32_t cvalid = min(32, min(p.block_n - ch * 32, p.ncols - col));  // valid columns of this chunk, >= 1
         __syncwarp();
@@ -227,6 +232,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const TileVar
                 }
             }
             if (ch + 1 < c_end) acc_ld32(arow, akey, ch + 1, acc);
+            if (ch + 2 == c_end) mbar_arrive(acc_empty);
             continue;
         }
         // ---- one chunk: alpha, column term, per-row time embedding, residual, packing, statistics, coalesced store.  The
@@ -247,7 +253,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const TileVar
                         q = make_uint4(0, 0, 0, 0);
                         if (ok_r && (lane & 3) * 8 + 8 <= cvalid) q = __ldg(reinterpret_cast<const uint4*>(res_lane + off_q[i] + col));
                     }
-                    sts128(w_res[i], q);
+                    sts128(w_res(i), q);
                 }
                 if ((FULL || res_pref) && ch + 1 < c_end) load_res(ch + 1, rq);
             }
@@ -277,7 +283,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const TileVar
             if (RES) {
 #pragma unroll
                 for (int j = 0; j < 4; ++j) {
-                    const uint4 q = lds128(r_res[j]);
+                    const uint4 q = lds128(r_res(j));
                     v[8 * j + 0] += bf16_lo(q.x); v[8 * j + 1] += bf16_hi(q.x);
                     v[8 * j + 2] += bf16_lo(q.y); v[8 * j + 3] += bf16_hi(q.y);
                     v[8 * j + 4] += bf16_lo(q.z); v[8 * j + 5] += bf16_hi(q.z);
@@ -294,13 +300,14 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const TileVar
                     q.y = pack_bf16(v[8 * j + 2], v[8 * j + 3]);
                     q.z = pack_bf16(v[8 * j + 4], v[8 * j + 5]);
                     q.w = pack_bf16(v[8 * j + 6], v[8 * j + 7]);
-                    sts128(w_own[j], q);
+                    sts128(w_own(j), q);
                 }
             } else {
 #pragma unroll
-                for (int j = 0; j < CPR; ++j) sts128(w_own[j], make_uint4(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]));
+                for (int j = 0; j < CPR; ++j) sts128(w_own(j), make_uint4(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]));
             }
             if (ch + 1 < c_end) acc_ld32(arow, akey, ch + 1, acc);   // next chunk
+            if (ch + 2 == c_end) mbar_arrive(acc_empty);             // ... the last one: the MMA warps may overwrite the tile
             __syncwarp();
             if (ESZ == 2 && STATS) {
                 // GroupNorm statistics of the tile just staged (the bf16 values the consumer will read): lanes 0-15 walk
@@ -334,7 +341,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const TileVar
 #pragma unroll
             for (int i = 0; i < CPR; ++i) {
                 if (!FULL && (!((ok_s >> i) & 1u) || nval <= 0)) continue;
-                const uint4 q = lds128(r_mov[i]);
+                const uint4 q = lds128(r_mov(i));
                 char* o = ob + off_s[i] * ESZ;
                 if (FULL || nval >= EPC) {
                     if (ESZ == 2 || p.out_mode == OUT_F32) {
@@ -376,9 +383,6 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const TileVar
             }
         }
     }
-    // row sums of operand A (weight gradient: the bias gradient).  Both warp pairs of a warpgroup see the same rows (they
-    // split the columns) - pair 0 alone adds them.
-    if (rowsum_tile && grp == 0 && row_ok) atomicAdd(p.rowsum + gw, rs_s[row]);
 }
 
 // One 64 x BN x 16 step of a consumer warpgroup.
@@ -454,19 +458,27 @@ __global__ void __launch_bounds__(kNumThreads, 1) gemm_tc_kernel(const __grid_co
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem_b + static_cast<size_t>(S) * p.stage_bytes_b);
     uint64_t* full_bar = bars;                       // [S]   TMA -> MMA
     uint64_t* empty_bar = bars + kMaxStages;         // [S]   MMA -> TMA
+    uint64_t* acc_full = bars + 2 * kMaxStages;      // accumulator tile written (MMA -> epilogue)
+    uint64_t* acc_empty = acc_full + 1;              // accumulator tile read (epilogue -> MMA)
     uint8_t* stg_base = reinterpret_cast<uint8_t*>(bars) + 256;               // epilogue staging tiles
     float* acc_f = reinterpret_cast<float*>(stg_base + kEpilogueStagingBytes);  // accumulator tile (acc_smem_bytes)
+    const uint32_t acc_pitch = static_cast<uint32_t>((p.block_n + 31) / 32 * 32);
+    const uint32_t acc_s = smem_u32(acc_f);
+    float* rs_s = acc_f + kBlockM * acc_pitch;   // EPI_ROWSUM_A: row sums of the tile
 
     const uint32_t warp = threadIdx.x >> 5;
     const uint32_t lane = lane_id();
+    const uint32_t wg = warp >> 2;
 
     if (warp == 8 && lane == 0) {
         tma_prefetch_desc(&p.a.map);
         tma_prefetch_desc(&p.b.map);
         for (int s = 0; s < S; ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 8);   // one arrival per consumer warp
+            mbar_init(&empty_bar[s], 8);   // one arrival per MMA warp
         }
+        mbar_init(acc_full, 256);          // every MMA thread, after its fragment stores
+        mbar_init(acc_empty, 128);         // every epilogue thread, after its last accumulator read
         fence_mbar_init();
     }
     if (rowsum_a && warp == 0) {   // the constant B operand of the row-sum MMAs; made visible to the tensor core (async proxy)
@@ -478,7 +490,8 @@ __global__ void __launch_bounds__(kNumThreads, 1) gemm_tc_kernel(const __grid_co
     __syncthreads();
     pdl_sync();  // the prologue above (barriers, descriptor prefetch) overlaps the tail of the previous kernel
 
-    if (warp >= 8) {
+    // Registers: 40 (producer) + 2 x 168 (MMA) + 136 (epilogue) per thread of each warpgroup = the whole 64 K register file
+    if (wg == 2) {
         // ------------------------------------------------------------------ TMA producer
         asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
         if (warp == 8 && elect_one()) {
@@ -525,13 +538,21 @@ __global__ void __launch_bounds__(kNumThreads, 1) gemm_tc_kernel(const __grid_co
                 }
             }
         }
+    } else if (wg == 3) {
+        // ------------------------------------------------------------------ epilogue warpgroup
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 136;");
+        uint32_t acc_phase = 0;
+        for (int32_t tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+            TileVars tv;
+            decompose_tile(p, tile, tv);
+            const bool rowsum_tile = rowsum_a && tv.t[0] == 0 && tv.t[2] == 0 && tv.t[3] == 0;
+            if (p.out_mode == OUT_BF16) epilogue_tile<2>(p, tv, rowsum_tile, warp & 3u, lane, acc_s, acc_pitch, smem_u32(rs_s), stg_base, acc_full, acc_empty, acc_phase);
+            else epilogue_tile<4>(p, tv, rowsum_tile, warp & 3u, lane, acc_s, acc_pitch, smem_u32(rs_s), stg_base, acc_full, acc_empty, acc_phase);
+            acc_phase ^= 1;
+        }
     } else {
-        // ------------------------------------------------------------------ consumer warpgroups: MMA, then epilogue
-        asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
-        const uint32_t wg = warp >> 2;
-        const uint32_t acc_pitch = static_cast<uint32_t>((p.block_n + 31) / 32 * 32);
-        const uint32_t acc_s = smem_u32(acc_f);
-        float* rs_s = acc_f + kBlockM * acc_pitch;   // EPI_ROWSUM_A: row sums of the tile
+        // ------------------------------------------------------------------ MMA warpgroups
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 168;");
         // this warpgroup's 64 rows of A: K-major, rows 64g.. (64 x 128 B further); MN-major, the g-th 64-wide box (8 KB)
         const uint32_t a_wg_off = wg * 8192u;
         // EPI_ROWSUM_A: D[64 x 16] += A_tile * ones: the same A descriptor against a K-major tile of ones (never advanced
@@ -540,8 +561,9 @@ __global__ void __launch_bounds__(kNumThreads, 1) gemm_tc_kernel(const __grid_co
         const bool release = lane == 0;
         const uint32_t a_base = smem_u32(smem_a) + a_wg_off, b_base = smem_u32(smem_b);
         Ring ring{0, 0};
+        uint32_t acc_phase = 0;
         for (int32_t tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-            float d[kMaxBlockN / 2];   // (declared per tile: dead during the epilogue)
+            float d[kMaxBlockN / 2];
             float drs[8];
             TileVars tv;
             decompose_tile(p, tile, tv);
@@ -565,7 +587,7 @@ __global__ void __launch_bounds__(kNumThreads, 1) gemm_tc_kernel(const __grid_co
             }
             // accumulator -> shared memory.  Fragment of m64nNk16: d[4j + 2h + e] is row 16 * (warp % 4) + lane / 4 + 8h,
             // column 8j + 2 * (lane % 4) + e.
-            named_bar_sync(1 + wg, 128);   // this warpgroup's epilogue of the previous tile has read its rows
+            mbar_wait(acc_empty, acc_phase ^ 1);   // the epilogue has read the previous tile (the first wait passes at once)
             {
                 const uint32_t r0 = wg * 64u + (warp & 3u) * 16u + (lane >> 2);
                 const uint32_t key = acc_swz(r0);   // == acc_swz(r0 + 8)
@@ -585,9 +607,8 @@ __global__ void __launch_bounds__(kNumThreads, 1) gemm_tc_kernel(const __grid_co
                     rs_s[r0 + 8] = drs[2];
                 }
             }
-            named_bar_sync(1 + wg, 128);
-            if (p.out_mode == OUT_BF16) epilogue_tile<2>(p, tv, rowsum_tile, warp, lane, acc_s, acc_pitch, rs_s, stg_base);
-            else epilogue_tile<4>(p, tv, rowsum_tile, warp, lane, acc_s, acc_pitch, rs_s, stg_base);
+            mbar_arrive(acc_full);
+            acc_phase ^= 1;
         }
     }
 }

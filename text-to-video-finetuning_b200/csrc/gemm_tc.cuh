@@ -20,12 +20,12 @@
 
 namespace t2v {
 
-constexpr int kBlockM = 128;      // two consumer warpgroups x wgmma M = 64
+constexpr int kBlockM = 128;      // two MMA warpgroups x wgmma M = 64
 constexpr int kBlockK = 64;       // bf16 elements per k-block (= one 128-byte swizzle row)
-constexpr int kMaxBlockN = 128;   // wgmma N; the fp32 accumulator (N / 2 registers per thread) must leave room for the epilogue
+constexpr int kMaxBlockN = 128;   // wgmma N; the fp32 accumulator is N / 2 registers per MMA thread
 constexpr int kMaxStages = 8;
-constexpr int kNumThreads = 384;  // warps 0-7: two MMA + epilogue warpgroups, warps 8-11: TMA producer (one lane)
-constexpr int kEpilogueStagingBytes = 8 * 4096 + 8 * 128;  // per epilogue warp: a 32-row x 128-byte staging tile + 32 bias floats
+constexpr int kNumThreads = 512;  // warps 0-7: two MMA warpgroups, warps 8-11: TMA producer (one lane), warps 12-15: epilogue
+constexpr int kEpilogueStagingBytes = 4 * 4096 + 4 * 128;  // per epilogue warp: a 32-row x 128-byte staging tile + 32 bias floats
 // The finished accumulator goes through shared memory ([128 rows][N rounded up to 32] fp32, plus 128 row sums) so that the
 // epilogue can own whole output rows.
 constexpr int acc_smem_bytes(int block_n) { return kBlockM * ((block_n + 31) / 32 * 32) * 4 + kBlockM * 4; }
