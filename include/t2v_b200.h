@@ -207,6 +207,11 @@ int t2v_nhwc8_to_latents(const void* in, float* out, int32_t B, int32_t C, int32
  * loss != NULL: *loss = mean((pred - target)^2).  dpred != NULL: dpred = *gout * 2 (pred - target) / numel.         */
 int t2v_mse_loss(const void* pred, const float* target, float* loss, const float* gout, void* dpred, int32_t B, int32_t C,
                  int32_t F, int32_t HW, void* stream);
+/* The same loss for a v-prediction model (train.py:792-800): the target is DDPMScheduler.get_velocity(x0, noise, t),
+ * sqrt(abar[t_b]) noise - sqrt(1 - abar[t_b]) x0, formed per element from the (B, C<=8, F, H, W) fp32 x0 and noise; it is
+ * never stored.  abar (fp32 [T]) and timesteps (int64 [B]) are read on the device.  loss / gout / dpred as t2v_mse_loss. */
+int t2v_velocity_mse_loss(const void* pred, const float* x0, const float* noise, const float* alphas_cumprod, const int64_t* timesteps,
+                          float* loss, const float* gout, void* dpred, int32_t B, int32_t C, int32_t F, int32_t HW, void* stream);
 
 /* AutoencoderKL latent_dist.sample() + rearrange + * scale (train.py:343-345): moments [B*F][HW][8] bf16 (mean | logvar),
  * eps (B,4,F,HW) fp32 -> out (B,4,F,HW) fp32 = (mean + exp(0.5 clamp(logvar,-30,20)) eps) * scale.                    */

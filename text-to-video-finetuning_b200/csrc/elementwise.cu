@@ -75,10 +75,15 @@ __global__ void from_nhwc8_kernel(const __nv_bfloat16* __restrict__ in, float* _
     }
 }
 
-// (B, C, F, H, W) fp32 gradient -> [B*F][H][W][8] bf16 scaled by *gscale (device scalar or NULL)
 // MSE forward: loss += sum (pred - target)^2 / numel ; backward: dpred = g * 2 (pred - target) / numel
-__global__ void mse_kernel(const __nv_bfloat16* __restrict__ pred, const float* __restrict__ target, float* __restrict__ loss,
-                           const float* __restrict__ gout, __nv_bfloat16* __restrict__ dpred, int B, int C, int F, int HW) {
+// target is (B, C, F, H, W) fp32.  With x0 given it is the noise of a v-prediction step and the regression target is the
+// velocity, formed per element and never stored:  v = sqrt(abar[t_b]) eps - sqrt(1 - abar[t_b]) x0  (DDPMScheduler.get_velocity,
+// train.py:796-797).  abar and t are read on the device, so a replayed CUDA graph uses each step's timesteps.
+// Six blocks per SM holds the kernel at the 40 registers the noise-target-only version used (no spills); left free, ptxas
+// keeps all sixteen loads of the velocity path in flight and takes 42, which drops a block per SM for both objectives.
+__global__ void __launch_bounds__(256, 6) mse_kernel(const __nv_bfloat16* __restrict__ pred, const float* __restrict__ target, float* __restrict__ loss,
+                           const float* __restrict__ gout, __nv_bfloat16* __restrict__ dpred, int B, int C, int F, int HW,
+                           const float* __restrict__ x0, const float* __restrict__ abar, const int64_t* __restrict__ t) {
     pdl_sync();
     const int64_t npix = int64_t(B) * F * HW;
     const float inv = 1.0f / (float(npix) * C);
@@ -88,12 +93,23 @@ __global__ void mse_kernel(const __nv_bfloat16* __restrict__ pred, const float* 
         const int hw = int(i % HW);
         const int f = int((i / HW) % F);
         const int b = int(i / (int64_t(HW) * F));
+        const int64_t src = (int64_t(b) * C * F + f) * HW + hw, cstride = int64_t(F) * HW;
+        float sa = 1.f, sb = 0.f;
+        if (x0) {
+            const float a = abar[t[b]];
+            sa = sqrtf(a);
+            sb = sqrtf(1.f - a);
+        }
         float v[8], d[8];
         unpack8e(__ldg(reinterpret_cast<const uint4*>(pred) + i), v);
 #pragma unroll
         for (int c = 0; c < 8; ++c) {
             float e = 0.f;
-            if (c < C) e = v[c] - target[((int64_t(b) * C + c) * F + f) * HW + hw];
+            if (c < C) {
+                float y = target[src + c * cstride];
+                if (x0) y = sa * y - sb * x0[src + c * cstride];
+                e = v[c] - y;
+            }
             acc += e * e;
             d[c] = 2.f * e * inv * g;
         }
@@ -556,8 +572,19 @@ int t2v_mse_loss(const void* pred, const float* target, float* loss, const float
                  int32_t F, int32_t HW, void* stream) {
     const int64_t n = int64_t(B) * F * HW;
     if (loss) cudaMemsetAsync(loss, 0, sizeof(float), ST);
-    launch_pdl(mse_kernel, dim3(ew_grid(n)), dim3(256), size_t(0), ST, BF(pred), target, loss, gout, BFW(dpred), B, C, F, HW);
+    launch_pdl(mse_kernel, dim3(ew_grid(n)), dim3(256), size_t(0), ST, BF(pred), target, loss, gout, BFW(dpred), B, C, F, HW,
+               (const float*)nullptr, (const float*)nullptr, (const int64_t*)nullptr);
     return launch_checked(int(cudaGetLastError()), "mse_loss");
+}
+int t2v_velocity_mse_loss(const void* pred, const float* x0, const float* noise, const float* alphas_cumprod, const int64_t* timesteps,
+                          float* loss, const float* gout, void* dpred, int32_t B, int32_t C, int32_t F, int32_t HW, void* stream) {
+    if (!x0 || !noise || !alphas_cumprod || !timesteps) return fail(-2, "velocity_mse_loss: x0, noise, alphas_cumprod and timesteps are required");
+    if (C > 8) return fail(-2, "velocity_mse_loss: C=%d > 8", C);
+    const int64_t n = int64_t(B) * F * HW;
+    if (loss) cudaMemsetAsync(loss, 0, sizeof(float), ST);
+    launch_pdl(mse_kernel, dim3(ew_grid(n)), dim3(256), size_t(0), ST, BF(pred), noise, loss, gout, BFW(dpred), B, C, F, HW, x0,
+               alphas_cumprod, timesteps);
+    return launch_checked(int(cudaGetLastError()), "velocity_mse_loss");
 }
 int t2v_geglu_fwd(const void* proj, void* out, int64_t M, int32_t I, void* stream) {
     if (I % 8) return fail(-2, "geglu: inner dim %d not a multiple of 8", I);

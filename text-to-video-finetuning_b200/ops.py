@@ -743,3 +743,22 @@ class _MseLoss(Function):
 
 def mse_loss_nhwc8(pred, target):
     return _MseLoss.apply(pred, target)
+
+
+class _VelocityMseLoss(Function):
+    """mean((pred - v)^2) in fp32 for a v-prediction model (train.py:792-800): the velocity target
+    sqrt(abar[t]) noise - sqrt(1 - abar[t]) x0 is formed inside the loss kernel, never stored."""
+
+    @staticmethod
+    def forward(ctx, pred, x0, noise, alphas_cumprod, timesteps):
+        ctx.save_for_backward(pred, x0, noise, alphas_cumprod, timesteps)
+        return prims.velocity_mse_loss_fwd(pred, x0, noise, alphas_cumprod, timesteps)
+
+    @staticmethod
+    def backward(ctx, g):
+        pred, x0, noise, abar, t = ctx.saved_tensors
+        return prims.velocity_mse_loss_bwd(pred, x0, noise, abar, t, _cont(g.float())), None, None, None, None
+
+
+def velocity_mse_loss_nhwc8(pred, x0, noise, alphas_cumprod, timesteps):
+    return _VelocityMseLoss.apply(pred, x0, noise, alphas_cumprod, timesteps)

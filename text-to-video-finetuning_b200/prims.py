@@ -562,3 +562,30 @@ def mse_loss_bwd(pred, target, gout):
     dpred = torch.empty_like(pred)
     native.check(native.lib().t2v_mse_loss(_p(pred), _p(target), _p(None), _p(gout), _p(dpred), B, C, F, H * W, _stream()))
     return dpred
+
+
+def _chk_velocity(pred, x0, noise, alphas_cumprod, timesteps):
+    _chk_bf16(pred)
+    _chk_f32(x0, noise, alphas_cumprod)
+    assert x0.shape == noise.shape and timesteps.dtype == torch.int64 and timesteps.is_cuda and timesteps.is_contiguous(), (
+        x0.shape, noise.shape, timesteps.dtype)
+    assert timesteps.shape == (x0.shape[0],), (timesteps.shape, x0.shape)
+
+
+def velocity_mse_loss_fwd(pred, x0, noise, alphas_cumprod, timesteps):
+    """mean((pred - v)^2), v = sqrt(abar[t]) noise - sqrt(1 - abar[t]) x0 formed in the kernel; pred [B*F,H,W,8] bf16."""
+    _chk_velocity(pred, x0, noise, alphas_cumprod, timesteps)
+    B, C, F, H, W = x0.shape
+    loss = torch.empty((), device=pred.device, dtype=torch.float32)
+    native.check(native.lib().t2v_velocity_mse_loss(_p(pred), _p(x0), _p(noise), _p(alphas_cumprod), _p(timesteps), _p(loss), _p(None),
+                                                    _p(None), B, C, F, H * W, _stream()))
+    return loss
+
+
+def velocity_mse_loss_bwd(pred, x0, noise, alphas_cumprod, timesteps, gout):
+    _chk_velocity(pred, x0, noise, alphas_cumprod, timesteps)
+    B, C, F, H, W = x0.shape
+    dpred = torch.empty_like(pred)
+    native.check(native.lib().t2v_velocity_mse_loss(_p(pred), _p(x0), _p(noise), _p(alphas_cumprod), _p(timesteps), _p(None), _p(gout),
+                                                    _p(dpred), B, C, F, H * W, _stream()))
+    return dpred

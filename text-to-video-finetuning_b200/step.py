@@ -1,6 +1,9 @@
 """Training-step glue of the hot path: the H100-native equivalents of the reference's
 `tensor_to_vae_latent` (train.py:339-347), `sample_noise` (:349-358), `noise_scheduler.add_noise` (:760) and the
-epsilon-MSE of `finetune_unet` (:720-836), plus the data-parallel step object used by train.py and bench.py."""
+epsilon / v-prediction MSE of `finetune_unet` (:720-836), the noise schedule of the checkpoint's scheduler config (:119), plus
+the data-parallel step object used by train.py and bench.py."""
+import json
+import math
 import os
 
 import torch
@@ -9,12 +12,66 @@ import torch.distributed as dist
 from . import ops, prims
 from .runtime import GradientBuckets, GraphedStep, ParamArena, allreduce_gradients
 
+PREDICTION_TYPES = ("epsilon", "v_prediction")
+BETA_SCHEDULES = ("linear", "scaled_linear", "squaredcos_cap_v2")
+
 
 def ddpm_alphas_cumprod(num_train_timesteps=1000, beta_start=0.00085, beta_end=0.012, device=None):
     """'scaled_linear' DDPM schedule of the ms-1.7b / zeroscope scheduler config (DDPMScheduler.alphas_cumprod)."""
     betas = torch.linspace(beta_start ** 0.5, beta_end ** 0.5, num_train_timesteps, dtype=torch.float32) ** 2
     a = torch.cumprod(1.0 - betas, dim=0)
     return a.to(device) if device is not None else a
+
+
+def _rescale_zero_terminal_snr(betas):
+    """Lin et al. 2023, 'Common Diffusion Noise Schedules and Sample Steps are Flawed', Algorithm 1: shift sqrt(abar) so its
+    last value is 0, scale it so its first value is unchanged, and rebuild the betas from ratios of consecutive abar."""
+    abar_sqrt = torch.cumprod(1.0 - betas, dim=0).sqrt()
+    first, last = abar_sqrt[0].clone(), abar_sqrt[-1].clone()
+    abar_sqrt = (abar_sqrt - last) * (first / (first - last))
+    abar = abar_sqrt ** 2
+    alphas = torch.cat([abar[0:1], abar[1:] / abar[:-1]])
+    return 1.0 - alphas
+
+
+def schedule_from_config(config):
+    """A diffusers scheduler config (the dict of scheduler/scheduler_config.json) -> (alphas_cumprod fp32 [T], prediction_type),
+    computed as DDPMScheduler.__init__ does (reference train.py:119 builds its DDPMScheduler from this file).  Missing keys
+    take the ms-1.7b / zeroscope values, so `{}` gives `ddpm_alphas_cumprod()`.  Keys it does not act on (clip_sample,
+    steps_offset, ...) only concern sampling; an unknown beta_schedule or prediction_type raises ValueError."""
+    cfg = dict(config or {})
+    prediction_type = cfg.get("prediction_type") or "epsilon"
+    if prediction_type not in PREDICTION_TYPES:
+        # 'sample' too: the reference's loss target (train.py:792-800) knows only these two
+        raise ValueError(f"prediction_type {prediction_type!r} is not supported; expected one of {PREDICTION_TYPES}")
+    T = int(cfg.get("num_train_timesteps", 1000))
+    beta_start, beta_end = float(cfg.get("beta_start", 0.00085)), float(cfg.get("beta_end", 0.012))
+    schedule = cfg.get("beta_schedule", "scaled_linear")
+    if cfg.get("trained_betas") is not None:
+        betas = torch.tensor(cfg["trained_betas"], dtype=torch.float32)
+    elif schedule == "linear":
+        betas = torch.linspace(beta_start, beta_end, T, dtype=torch.float32)
+    elif schedule == "scaled_linear":
+        betas = torch.linspace(beta_start ** 0.5, beta_end ** 0.5, T, dtype=torch.float32) ** 2
+    elif schedule == "squaredcos_cap_v2":
+        def abar(s):
+            return math.cos((s + 0.008) / 1.008 * math.pi / 2) ** 2
+        betas = torch.tensor([min(1 - abar((i + 1) / T) / abar(i / T), 0.999) for i in range(T)], dtype=torch.float32)
+    else:
+        raise ValueError(f"beta_schedule {schedule!r} is not supported; expected one of {BETA_SCHEDULES}")
+    if cfg.get("rescale_betas_zero_snr", False):
+        betas = _rescale_zero_terminal_snr(betas)
+    return torch.cumprod(1.0 - betas, dim=0), prediction_type
+
+
+def load_noise_schedule(pretrained_model_path):
+    """(alphas_cumprod, prediction_type) of `<pretrained_model_path>/scheduler/scheduler_config.json`; a folder without that
+    file (a UNet-only checkpoint) gets the ms-1.7b / zeroscope defaults, `ddpm_alphas_cumprod()` and 'epsilon'."""
+    path = os.path.join(pretrained_model_path, "scheduler", "scheduler_config.json")
+    if not os.path.isfile(path):
+        return ddpm_alphas_cumprod(), "epsilon"
+    with open(path) as f:
+        return schedule_from_config(json.load(f))
 
 
 def sample_noise(latents, noise_strength=0.0, use_offset_noise=False, generator=None):
@@ -26,16 +83,23 @@ def sample_noise(latents, noise_strength=0.0, use_offset_noise=False, generator=
     return noise
 
 
-def finetune_loss(unet, latents, noise, timesteps, encoder_hidden_states, alphas_cumprod, return_pred=False):
-    """One UNet pass of finetune_unet for prediction_type 'epsilon':
-       noisy = add_noise(latents, noise, t)  ->  pred = unet(noisy, t, text)  ->  mse(pred.float(), noise.float()).
+def finetune_loss(unet, latents, noise, timesteps, encoder_hidden_states, alphas_cumprod, return_pred=False, prediction_type="epsilon"):
+    """One UNet pass of finetune_unet:
+       noisy = add_noise(latents, noise, t)  ->  pred = unet(noisy, t, text)  ->  mse(pred.float(), target.float())
+    with target = noise for prediction_type 'epsilon' and get_velocity(latents, noise, t) for 'v_prediction' (train.py:792-800).
     add_noise is fused into the layout-conversion kernel at the input, the loss reads the channels-last prediction
-    directly, so no (B,C,F,H,W) activation is ever materialised."""
+    directly (and forms the velocity per element), so no (B,C,F,H,W) activation is ever materialised."""
+    if prediction_type not in PREDICTION_TYPES:
+        raise ValueError(f"prediction_type {prediction_type!r} is not supported; expected one of {PREDICTION_TYPES}")
     B, C, F, H, W = latents.shape
     x = prims.latents_to_nhwc8(latents.float().contiguous(), noise.float().contiguous(), alphas_cumprod, timesteps.to(torch.int64).contiguous())
     text = unet.prepare_text(encoder_hidden_states)
     pred = unet.forward_channels_last(x, timesteps.to(torch.int64).contiguous(), text, B, F)
-    loss = ops.mse_loss_nhwc8(pred, noise.float().contiguous())
+    if prediction_type == "v_prediction":
+        loss = ops.velocity_mse_loss_nhwc8(pred, latents.float().contiguous(), noise.float().contiguous(), alphas_cumprod,
+                                           timesteps.to(torch.int64).contiguous())
+    else:
+        loss = ops.mse_loss_nhwc8(pred, noise.float().contiguous())
     if return_pred:
         return loss, prims.nhwc8_to_latents(pred.detach(), B, C, F)
     return loss
@@ -55,11 +119,17 @@ class DataParallelStep:
       * the all-reduce runs only on the window's last micro-step;
       * with an attached optim.FusedAdamW the update kernel consumes and zeroes the gradients and rewrites the bf16 shadow,
         so neither a memset nor a cast pass remains in the step.  Without one (a torch optimizer, or fwd+bwd only) the
-        buffer is zeroed at the start of each window and the shadow is re-cast from the masters every call."""
+        buffer is zeroed at the start of each window and the shadow is re-cast from the masters every call.
 
-    def __init__(self, unet, alphas_cumprod, passes=1, use_graph=False, adopt=True, optimizer=None, accumulation=1):
+    `prediction_type` picks the loss target of every pass: the noise ('epsilon') or the velocity ('v_prediction')."""
+
+    def __init__(self, unet, alphas_cumprod, passes=1, use_graph=False, adopt=True, optimizer=None, accumulation=1,
+                 prediction_type="epsilon"):
+        if prediction_type not in PREDICTION_TYPES:
+            raise ValueError(f"prediction_type {prediction_type!r} is not supported; expected one of {PREDICTION_TYPES}")
         self.unet = unet
         self.abar = alphas_cumprod
+        self.prediction_type = prediction_type
         self.passes = passes
         self.arena = ParamArena(unet) if adopt else None
         self.use_graph = use_graph
@@ -97,7 +167,7 @@ class DataParallelStep:
         reduce_now = last and self.sync_gradients
         overlap = self.buckets is not None and reduce_now
         for i in range(self.passes):
-            loss = finetune_loss(self.unet, latents, noise, timesteps, text, self.abar)
+            loss = finetune_loss(self.unet, latents, noise, timesteps, text, self.abar, prediction_type=self.prediction_type)
             if overlap:
                 self.buckets.armed = i == self.passes - 1   # gradients are final only in the last pass
             loss.backward(self._gscale if self.accumulation > 1 else None)

@@ -28,7 +28,7 @@ import torch
 import torch.distributed as dist
 
 from .models.unet_3d_condition import UNet3DConditionModel
-from .step import DataParallelStep, ddpm_alphas_cumprod, sample_noise
+from .step import DataParallelStep, load_noise_schedule, sample_noise
 from .utils.lora_handler import LORA_VERSIONS, LoraHandler
 
 already_printed_trainables = False
@@ -247,6 +247,9 @@ def main(
     fused_adamw = bool(kwargs.get("fused_adamw", True))   # optim.FusedAdamW on the flat arena (SURVEY 8(f) row 1); False: torch AdamW
     if use_8bit_adam and not fused_adamw:
         raise ValueError("use_8bit_adam runs optim.AdamW8bit on the flat arena; it cannot be combined with fused_adamw=False")
+    # noise schedule and loss target of the checkpoint (train.py:119, 792-800); an unsupported config fails here, before any
+    # weights move.  `rescale_schedule` stays a no-op: in the reference it never reaches add_noise (SURVEY H5).
+    abar, prediction_type = load_noise_schedule(pretrained_model_path)
     if seed is not None:
         # model construction and LoRA initialisation (lora_down ~ N(0, 1/r)) must be identical on every rank: the reference
         # gets that from accelerate/DDP broadcasting rank 0's parameters at wrap time (train.py:661).  The per-rank stream
@@ -279,9 +282,10 @@ def main(
         param_optim(unet_lora_params, use_unet_lora, is_lora=True, extra_params={**{"lr": learning_rate}, **extra_unet_params}),
     ], learning_rate)
 
-    abar = ddpm_alphas_cumprod(device=dev)
+    abar = abar.to(dev)
     use_graph = bool(kwargs.get("use_cuda_graph", dev.type == "cuda"))   # replay the whole step as one CUDA graph (static shapes)
-    stepper = DataParallelStep(unet, abar, passes=2, use_graph=use_graph, accumulation=gradient_accumulation_steps)
+    stepper = DataParallelStep(unet, abar, passes=2, use_graph=use_graph, accumulation=gradient_accumulation_steps,
+                               prediction_type=prediction_type)
     # parameters now live in the flat arena.  Every rank must start from rank 0's weights (DDP does this at wrap time).
     if world > 1:
         dist.broadcast(stepper.arena.master, src=0)
@@ -398,7 +402,8 @@ def main(
                     and text_encoder is not None and tokenizer is not None and getattr(vae, "decoder", None) is not None:
                 from .sampling import validation_sample
                 validation_sample(unet, vae, text_encoder, tokenizer, validation_data, os.path.join(output_dir, "samples"), global_step,
-                                  batch.get("text_prompt", [""])[0] if isinstance(batch.get("text_prompt"), (list, tuple)) else "", dev)
+                                  batch.get("text_prompt", [""])[0] if isinstance(batch.get("text_prompt"), (list, tuple)) else "", dev,
+                                  alphas_cumprod=abar, prediction_type=prediction_type)
             if global_step >= max_train_steps:
                 break
     if world > 1:
