@@ -285,6 +285,15 @@ int t2v_attn_small_fwd(const void* q, const void* k, const void* v, void* o, int
 int t2v_attn_small_bwd(const void* q, const void* k, const void* v, const void* dout, void* dq, void* dk, void* dv, int64_t nseq,
                        int32_t inner, int64_t outer_rows, int64_t inner_rows, int64_t seq_rows, int64_t ld_in, int64_t ld_out,
                        int32_t heads, int32_t L, int32_t D, void* stream);
+/* The same attention for 1 <= L <= 256 (clips longer than 32 frames), one CTA per (sequence, head), same addressing and
+ * head_dim.  The forward also writes lse: fp32 [nseq][heads][L], the natural-log logsumexp of each row of scaled scores.
+ * The backward reads lse and the forward's o (delta = rowsum(dout * o)); it is one pass without atomics and deterministic.  */
+int t2v_attn_long_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int64_t nseq, int32_t inner, int64_t outer_rows,
+                      int64_t inner_rows, int64_t seq_rows, int64_t ld_in, int64_t ld_out, int32_t heads, int32_t L, int32_t D,
+                      void* stream);
+int t2v_attn_long_bwd(const void* q, const void* k, const void* v, const void* o, const void* dout, const float* lse, void* dq, void* dk,
+                      void* dv, int64_t nseq, int32_t inner, int64_t outer_rows, int64_t inner_rows, int64_t seq_rows, int64_t ld_in,
+                      int64_t ld_out, int32_t heads, int32_t L, int32_t D, void* stream);
 
 /* Fused AdamW + global-norm clipping on the flat arena (torch.optim.AdamW semantics; reference train.py:616-623, clipping
  * :868-876).  The trainable set is a chunk table of int64 (offset, length) pairs into the flat fp32 buffers (multiples of 64

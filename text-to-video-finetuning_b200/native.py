@@ -80,6 +80,7 @@ EXPORTS = [
     "t2v_silu_bwd_f32", "t2v_silu_bf16", "t2v_silu_bf16_bwd", "t2v_add_bf16", "t2v_add_f32", "t2v_dropout_scale_add", "t2v_scale_bf16", "t2v_cast_f32_bf16", "t2v_embed_tokens", "t2v_gelu_bf16", "t2v_frames_u8_to_nhwc8", "t2v_scale_cast_f32_bf16", "t2v_cast_bf16_f32", "t2v_sqnorm_chunks", "t2v_adamw_prepare", "t2v_adamw_chunks", "t2v_adamw8bit_chunks", "t2v_counter_add", "t2v_upsample_nearest_fwd",
     "t2v_upsample_nearest_bwd", "t2v_copy_cols", "t2v_colsum", "t2v_colsum_f32", "t2v_softmax_fwd", "t2v_softmax_bwd",
     "t2v_timestep_embedding", "t2v_attn_small_fwd", "t2v_attn_small_bwd",
+    "t2v_attn_long_fwd", "t2v_attn_long_bwd",
 ]
 
 
@@ -146,6 +147,8 @@ def _declare(lib):
     lib.t2v_timestep_embedding.argtypes = [vp, vp, i32, i32, vp]
     lib.t2v_attn_small_fwd.argtypes = [vp] * 4 + [i64, i32, i64, i64, i64, i64, i64, i32, i32, i32, vp]
     lib.t2v_attn_small_bwd.argtypes = [vp] * 7 + [i64, i32, i64, i64, i64, i64, i64, i32, i32, i32, vp]
+    lib.t2v_attn_long_fwd.argtypes = [vp] * 5 + [i64, i32, i64, i64, i64, i64, i64, i32, i32, i32, vp]
+    lib.t2v_attn_long_bwd.argtypes = [vp] * 9 + [i64, i32, i64, i64, i64, i64, i64, i32, i32, i32, vp]
     for name in EXPORTS:
         getattr(lib, name)  # every declared symbol must be exported
     return lib

@@ -668,9 +668,14 @@ def _temporal_addr(B, F, HW, heads, D, ld_in, ld_out):
     return (B * HW, HW, F * HW, 1, HW, ld_in, ld_out, heads, F, D)
 
 
+SMALL_TEMPORAL_MAX = 32   # clips of up to this many frames use attn_small (a warp per sequence); longer ones attn_long
+MAX_FRAMES = 256          # attn_long keeps a whole sequence of q, k, v, dO in one CTA's shared memory
+
+
 class _TemporalAttention(Function):
     """Self-attention along the frame axis on frames-major tokens [B*F*HW, H*D] (no permute; see attn_small.cu).
-    `fused`: q is the [rows, 3C] QKV projection and k, v are None."""
+    `fused`: q is the [rows, 3C] QKV projection and k, v are None.  F <= 32 runs attn_small; 32 < F <= 256 runs attn_long,
+    whose backward also needs the forward's o and row logsumexp."""
 
     @staticmethod
     def forward(ctx, q, k, v, heads, B, F, HW, fused):
@@ -682,22 +687,32 @@ class _TemporalAttention(Function):
             qq, kk, vv = q, k, v
         addr = _temporal_addr(B, F, HW, heads, C // heads, q.shape[-1], C)
         o = torch.empty((q.shape[0], C), device=q.device, dtype=q.dtype)
-        prims.attn_small_fwd(qq, kk, vv, o, addr)
-        ctx.addr, ctx.fused = addr, fused
-        ctx.save_for_backward(q, k, v)
+        ctx.addr, ctx.fused, ctx.long = addr, fused, F > SMALL_TEMPORAL_MAX
+        if ctx.long:
+            lse = torch.empty((B * HW, heads, F), device=q.device, dtype=torch.float32)
+            prims.attn_long_fwd(qq, kk, vv, o, lse, addr)
+            ctx.save_for_backward(q, k, v, o, lse)
+        else:
+            prims.attn_small_fwd(qq, kk, vv, o, addr)
+            ctx.save_for_backward(q, k, v)
         return o
 
     @staticmethod
     def backward(ctx, do):
-        q, k, v = ctx.saved_tensors
+        if ctx.long:
+            q, k, v, o, lse = ctx.saved_tensors
+            bwd = lambda q_, k_, v_, do_, dq_, dk_, dv_, addr: prims.attn_long_bwd(q_, k_, v_, o, do_, lse, dq_, dk_, dv_, addr)
+        else:
+            q, k, v = ctx.saved_tensors
+            bwd = prims.attn_small_bwd
         do = _cont(do)
         if ctx.fused:
             C = q.shape[-1] // 3
             dqkv = torch.empty_like(q)
-            prims.attn_small_bwd(q[:, :C], q[:, C:2 * C], q[:, 2 * C:], do, dqkv[:, :C], dqkv[:, C:2 * C], dqkv[:, 2 * C:], ctx.addr)
+            bwd(q[:, :C], q[:, C:2 * C], q[:, 2 * C:], do, dqkv[:, :C], dqkv[:, C:2 * C], dqkv[:, 2 * C:], ctx.addr)
             return dqkv, None, None, None, None, None, None, None
         dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
-        prims.attn_small_bwd(q, k, v, do, dq, dk, dv, ctx.addr)
+        bwd(q, k, v, do, dq, dk, dv, ctx.addr)
         return dq, dk, dv, None, None, None, None, None
 
 

@@ -514,6 +514,23 @@ def attn_small_bwd(q, k, v, do, dq, dk, dv, addr):
     return dq, dk, dv
 
 
+def attn_long_fwd(q, k, v, o, lse, addr):
+    """attn_small_fwd for 1 <= L <= 256; also writes lse fp32 [nseq, heads, L] (natural-log row logsumexp of the scaled
+    scores), which attn_long_bwd reads."""
+    _chk_rows_bf16(q, k, v, o)
+    _chk_f32(lse)
+    native.check(native.lib().t2v_attn_long_fwd(_p(q), _p(k), _p(v), _p(o), _p(lse), *addr, _stream()))
+    return o, lse
+
+
+def attn_long_bwd(q, k, v, o, do, lse, dq, dk, dv, addr):
+    """o / lse: the forward's outputs (delta = rowsum(dO o O) is formed from o)."""
+    _chk_rows_bf16(q, k, v, o, do, dq, dk, dv)
+    _chk_f32(lse)
+    native.check(native.lib().t2v_attn_long_bwd(_p(q), _p(k), _p(v), _p(o), _p(do), _p(lse), _p(dq), _p(dk), _p(dv), *addr, _stream()))
+    return dq, dk, dv
+
+
 def timestep_embedding(t, dim):
     assert t.dtype == torch.int64 and t.is_cuda
     out = torch.empty((t.shape[0], dim), device=t.device, dtype=torch.bfloat16)

@@ -28,6 +28,7 @@ import torch
 import torch.distributed as dist
 
 from .models.unet_3d_condition import UNet3DConditionModel
+from .ops import MAX_FRAMES
 from .step import DataParallelStep, load_noise_schedule, sample_noise
 from .utils.lora_handler import LORA_VERSIONS, LoraHandler
 
@@ -250,6 +251,11 @@ def main(
     # noise schedule and loss target of the checkpoint (train.py:119, 792-800); an unsupported config fails here, before any
     # weights move.  `rescale_schedule` stays a no-op: in the reference it never reaches add_noise (SURVEY H5).
     abar, prediction_type = load_noise_schedule(pretrained_model_path)
+    # temporal attention runs on clips of 1..256 frames (attn_small.cu); a longer clip fails here, not in the first step
+    for section, key, data in (("train_data", "n_sample_frames", train_data), ("validation_data", "num_frames", validation_data)):
+        frames = int((data or {}).get(key, 16))
+        if frames > MAX_FRAMES:
+            raise ValueError(f"{section}.{key} = {frames}: temporal attention supports at most {MAX_FRAMES} frames")
     if seed is not None:
         # model construction and LoRA initialisation (lora_down ~ N(0, 1/r)) must be identical on every rank: the reference
         # gets that from accelerate/DDP broadcasting rank 0's parameters at wrap time (train.py:661).  The per-rank stream
