@@ -325,6 +325,24 @@ int t2v_adamw8bit_chunks(float* p, float* g, const void* g_bf16, void* shadow_bf
                          const float* hp, const float* qmaps, float* m32, float* v32, void* code_m, void* code_v, float* absmax_m,
                          float* absmax_v, int32_t zero_grad, void* stream);
 
+/* Exponential moving average of the trained weights (`use_ema`; diffusers' EMAModel with its default arguments), updated in
+ * the same pass as the weights.  k = *step, the step count after t2v_adamw_prepare's increment, read on the device so that a
+ * replayed CUDA graph uses each step's decay: d = 0 for k = 1, else min(ema_decay, k / (9 + k)) (fp64); then per element
+ * ema -= (1 - d) * (ema - p_new), with 1 - d rounded to fp32 and each operation rounded on its own.  ema (fp32, 16-byte
+ * aligned) is compact: the EMA offset column of each row says where its elements start.  ema_decay must lie in [0, 1].
+ *   t2v_adamw_ema_chunks      t2v_adamw_chunks with rows (arena offset, length, EMA offset)
+ *   t2v_adamw8bit_ema_chunks  t2v_adamw8bit_chunks with rows (arena offset, length, state offset, bits, EMA offset); both the
+ *                             32-bit and the 8-bit rows update the fp32 EMA
+ *   t2v_ema_swap_chunks       exchanges p and ema over n_rows rows (arena offset, length, EMA offset) and rewrites the bf16
+ *                             copy of p for offsets < n_shadow as the update kernels round it; a second call restores all
+ *                             three bit for bit                                                                          */
+int t2v_adamw_ema_chunks(float* p, float* g, const void* g_bf16, float* m, float* v, void* shadow_bf16, int64_t n_shadow, const int64_t* chunks,
+                         int32_t n_chunks, const float* hp, int32_t zero_grad, float* ema, const int64_t* step, float ema_decay, void* stream);
+int t2v_adamw8bit_ema_chunks(float* p, float* g, const void* g_bf16, void* shadow_bf16, int64_t n_shadow, const int64_t* chunks, int32_t n_chunks,
+                             const float* hp, const float* qmaps, float* m32, float* v32, void* code_m, void* code_v, float* absmax_m,
+                             float* absmax_v, int32_t zero_grad, float* ema, const int64_t* step, float ema_decay, void* stream);
+int t2v_ema_swap_chunks(float* p, float* ema, void* shadow_bf16, int64_t n_shadow, const int64_t* rows, int32_t n_rows, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -51,11 +51,31 @@ __device__ __forceinline__ AdamWArgs load_hp(const float* hp) {
     return a;
 }
 
+// Exponential moving average of the updated weights (diffusers' EMAModel with its default arguments).  k = the step count
+// after this step's increment (adamw_prepare): d_1 = 0, d_k = min(decay, k / (9 + k)) for k >= 2, computed in fp64; the
+// kernels use 1 - d_k rounded to fp32.  The lerp is EMAModel.step's `s -= (1 - d) * (s - p)`, each operation rounded on its
+// own (no FMA contraction), so it restates torch's fp32 arithmetic exactly.
+__device__ __forceinline__ float ema_one_minus_decay(const int64_t* __restrict__ step, float decay) {
+    const double k = double(*step);
+    const double d = k <= 1.0 ? 0.0 : fmin(double(decay), k / (9.0 + k));
+    return float(1.0 - d);
+}
+
+__device__ __forceinline__ void ema_lerp(float4& e, const float4& p, float omd) {
+    e.x = __fsub_rn(e.x, __fmul_rn(omd, __fsub_rn(e.x, p.x)));
+    e.y = __fsub_rn(e.y, __fmul_rn(omd, __fsub_rn(e.y, p.y)));
+    e.z = __fsub_rn(e.z, __fmul_rn(omd, __fsub_rn(e.z, p.z)));
+    e.w = __fsub_rn(e.w, __fmul_rn(omd, __fsub_rn(e.w, p.w)));
+}
+
 // One chunk with fp32 state, the block's threads striding over it: elements [off, off + len) of p, g, shadow (written when sh)
-// and g16 (may be NULL), state elements [soff, soff + len) of m and v.
+// and g16 (may be NULL), state elements [soff, soff + len) of m and v.  kEma: then also the EMA elements [eoff, eoff + len),
+// lerped towards the new p with omd = 1 - d_k.
+template <bool kEma>
 __device__ __forceinline__ void adamw_chunk_f32(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
                                                 __nv_bfloat16* __restrict__ shadow, bool sh, const __nv_bfloat16* __restrict__ g16,
-                                                int64_t off, int64_t soff, int64_t len, const AdamWArgs& a, int zero_grad) {
+                                                int64_t off, int64_t soff, int64_t len, const AdamWArgs& a, int zero_grad,
+                                                float* __restrict__ ema, int64_t eoff, float omd) {
     float4* p4 = reinterpret_cast<float4*>(p + off);
     float4* g4 = reinterpret_cast<float4*>(g + off);
     float4* m4 = reinterpret_cast<float4*>(m + soff);
@@ -81,6 +101,12 @@ __device__ __forceinline__ void adamw_chunk_f32(float* __restrict__ p, float* __
         p4[i] = pp;
         m4[i] = mm;
         v4[i] = vv;
+        if constexpr (kEma) {
+            float4* e4 = reinterpret_cast<float4*>(ema + eoff);
+            float4 ee = e4[i];
+            ema_lerp(ee, pp, omd);
+            e4[i] = ee;
+        }
         if (sh) {
             uint2 q;
             q.x = pack_bf16(pp.x, pp.y);
@@ -92,18 +118,39 @@ __device__ __forceinline__ void adamw_chunk_f32(float* __restrict__ p, float* __
 }
 
 // g16 != NULL: the gradient comes from the bf16 communication buffer (the all-reduced, averaged gradient of a data-parallel
-// step); the fp32 accumulation buffer g is then only zeroed.
+// step); the fp32 accumulation buffer g is then only zeroed.  Chunk rows: (offset, length), or with kEma (offset, length,
+// EMA offset).
+template <bool kEma>
+__device__ __forceinline__ void adamw_chunks_body(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
+                                                  __nv_bfloat16* __restrict__ shadow, int64_t n_shadow, const int64_t* __restrict__ chunks,
+                                                  int n_chunks, const float* __restrict__ hp, int zero_grad,
+                                                  const __nv_bfloat16* __restrict__ g16, float* __restrict__ ema,
+                                                  const int64_t* __restrict__ step, float ema_decay) {
+    constexpr int kCols = kEma ? 3 : 2;
+    pdl_sync();
+    const AdamWArgs a = load_hp(hp);
+    float omd = 0.f;
+    if constexpr (kEma) omd = ema_one_minus_decay(step, ema_decay);
+    for (int c = blockIdx.x; c < n_chunks; c += gridDim.x) {
+        const int64_t off = chunks[kCols * c], len = chunks[kCols * c + 1];
+        const bool sh = shadow != nullptr && off < n_shadow;
+        adamw_chunk_f32<kEma>(p, g, m, v, shadow, sh, g16, off, off, len, a, zero_grad, ema, kEma ? chunks[kCols * c + kCols - 1] : 0, omd);
+    }
+}
+
 __global__ void __launch_bounds__(256) adamw_chunks_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m,
                                                            float* __restrict__ v, __nv_bfloat16* __restrict__ shadow, int64_t n_shadow,
                                                            const int64_t* __restrict__ chunks, int n_chunks, const float* __restrict__ hp,
                                                            int zero_grad, const __nv_bfloat16* __restrict__ g16) {
-    pdl_sync();
-    const AdamWArgs a = load_hp(hp);
-    for (int c = blockIdx.x; c < n_chunks; c += gridDim.x) {
-        const int64_t off = chunks[2 * c], len = chunks[2 * c + 1];
-        const bool sh = shadow != nullptr && off < n_shadow;
-        adamw_chunk_f32(p, g, m, v, shadow, sh, g16, off, off, len, a, zero_grad);
-    }
+    adamw_chunks_body<false>(p, g, m, v, shadow, n_shadow, chunks, n_chunks, hp, zero_grad, g16, nullptr, nullptr, 0.f);
+}
+
+__global__ void __launch_bounds__(256) adamw_ema_chunks_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m,
+                                                               float* __restrict__ v, __nv_bfloat16* __restrict__ shadow, int64_t n_shadow,
+                                                               const int64_t* __restrict__ chunks, int n_chunks, const float* __restrict__ hp,
+                                                               int zero_grad, const __nv_bfloat16* __restrict__ g16, float* __restrict__ ema,
+                                                               const int64_t* __restrict__ step, float ema_decay) {
+    adamw_chunks_body<true>(p, g, m, v, shadow, n_shadow, chunks, n_chunks, hp, zero_grad, g16, ema, step, ema_decay);
 }
 
 // Blockwise 8-bit AdamW (optim.AdamW8bit; Dettmers et al., ICLR 2022).  Chunk rows are int64 quadruples (arena offset, length,
@@ -125,12 +172,16 @@ __device__ __forceinline__ uint32_t quantize(float x, float absmax, const float*
     return k - 256;
 }
 
-__global__ void __launch_bounds__(256) adamw8bit_chunks_kernel(float* __restrict__ p, float* __restrict__ g, __nv_bfloat16* __restrict__ shadow,
-                                                               int64_t n_shadow, const int64_t* __restrict__ chunks, int n_chunks,
-                                                               const float* __restrict__ hp, const float* __restrict__ qmaps, float* __restrict__ m32,
-                                                               float* __restrict__ v32, uint8_t* __restrict__ qm, uint8_t* __restrict__ qv,
-                                                               float* __restrict__ absmax_m, float* __restrict__ absmax_v, int zero_grad,
-                                                               const __nv_bfloat16* __restrict__ g16) {
+// kEma: rows carry a fifth column, the EMA offset; both the 32-bit and the 8-bit rows lerp the fp32 EMA towards the new p.
+template <bool kEma>
+__device__ __forceinline__ void adamw8bit_chunks_body(float* __restrict__ p, float* __restrict__ g, __nv_bfloat16* __restrict__ shadow,
+                                                      int64_t n_shadow, const int64_t* __restrict__ chunks, int n_chunks,
+                                                      const float* __restrict__ hp, const float* __restrict__ qmaps, float* __restrict__ m32,
+                                                      float* __restrict__ v32, uint8_t* __restrict__ qm, uint8_t* __restrict__ qv,
+                                                      float* __restrict__ absmax_m, float* __restrict__ absmax_v, int zero_grad,
+                                                      const __nv_bfloat16* __restrict__ g16, float* __restrict__ ema,
+                                                      const int64_t* __restrict__ step, float ema_decay) {
+    constexpr int kCols = kEma ? 5 : 4;
     __shared__ float map_m[256], map_v[256], tree_m[256], tree_v[256];
     __shared__ uint32_t zero_m;
     pdl_sync();
@@ -148,12 +199,15 @@ __global__ void __launch_bounds__(256) adamw8bit_chunks_kernel(float* __restrict
     __syncthreads();
     const uint32_t zm = zero_m, zv = 0;   // the unsigned map starts at 0.0
     const AdamWArgs a = load_hp(hp);
+    float omd = 0.f;
+    if constexpr (kEma) omd = ema_one_minus_decay(step, ema_decay);
     const int lane = t & 31, warp = t >> 5;
     for (int c = blockIdx.x; c < n_chunks; c += gridDim.x) {
-        const int64_t off = chunks[4 * c], len = chunks[4 * c + 1], soff = chunks[4 * c + 2];
+        const int64_t off = chunks[kCols * c], len = chunks[kCols * c + 1], soff = chunks[kCols * c + 2];
+        const int64_t eoff = kEma ? chunks[kCols * c + kCols - 1] : 0;
         const bool sh = shadow != nullptr && off < n_shadow;
-        if (chunks[4 * c + 3] != 8) {   // uniform across the thread block
-            adamw_chunk_f32(p, g, m32, v32, shadow, sh, g16, off, soff, len, a, zero_grad);
+        if (chunks[kCols * c + 3] != 8) {   // uniform across the thread block
+            adamw_chunk_f32<kEma>(p, g, m32, v32, shadow, sh, g16, off, soff, len, a, zero_grad, ema, eoff, omd);
             continue;
         }
         const int nblk = int((len + kQBlock - 1) / kQBlock);
@@ -220,12 +274,62 @@ __global__ void __launch_bounds__(256) adamw8bit_chunks_kernel(float* __restrict
                 }
                 *reinterpret_cast<uint32_t*>(qm + soff + e0 + j) = cm;
                 *reinterpret_cast<uint32_t*>(qv + soff + e0 + j) = cv;
-                *reinterpret_cast<float4*>(p + e) = make_float4(pe[4 * h], pe[4 * h + 1], pe[4 * h + 2], pe[4 * h + 3]);
+                const float4 pn = make_float4(pe[4 * h], pe[4 * h + 1], pe[4 * h + 2], pe[4 * h + 3]);
+                *reinterpret_cast<float4*>(p + e) = pn;
+                if constexpr (kEma) {
+                    float4* e4 = reinterpret_cast<float4*>(ema + eoff + e0 + j);
+                    float4 ee = *e4;
+                    ema_lerp(ee, pn, omd);
+                    *e4 = ee;
+                }
                 if (sh)
                     *reinterpret_cast<uint2*>(shadow + e) =
                         make_uint2(pack_bf16(pe[4 * h], pe[4 * h + 1]), pack_bf16(pe[4 * h + 2], pe[4 * h + 3]));
                 if (zero_grad) *reinterpret_cast<float4*>(g + e) = make_float4(0.f, 0.f, 0.f, 0.f);
             }
+        }
+    }
+}
+
+__global__ void __launch_bounds__(256) adamw8bit_chunks_kernel(float* __restrict__ p, float* __restrict__ g, __nv_bfloat16* __restrict__ shadow,
+                                                               int64_t n_shadow, const int64_t* __restrict__ chunks, int n_chunks,
+                                                               const float* __restrict__ hp, const float* __restrict__ qmaps, float* __restrict__ m32,
+                                                               float* __restrict__ v32, uint8_t* __restrict__ qm, uint8_t* __restrict__ qv,
+                                                               float* __restrict__ absmax_m, float* __restrict__ absmax_v, int zero_grad,
+                                                               const __nv_bfloat16* __restrict__ g16) {
+    adamw8bit_chunks_body<false>(p, g, shadow, n_shadow, chunks, n_chunks, hp, qmaps, m32, v32, qm, qv, absmax_m, absmax_v, zero_grad, g16,
+                                 nullptr, nullptr, 0.f);
+}
+
+__global__ void __launch_bounds__(256) adamw8bit_ema_chunks_kernel(float* __restrict__ p, float* __restrict__ g, __nv_bfloat16* __restrict__ shadow,
+                                                                   int64_t n_shadow, const int64_t* __restrict__ chunks, int n_chunks,
+                                                                   const float* __restrict__ hp, const float* __restrict__ qmaps,
+                                                                   float* __restrict__ m32, float* __restrict__ v32, uint8_t* __restrict__ qm,
+                                                                   uint8_t* __restrict__ qv, float* __restrict__ absmax_m,
+                                                                   float* __restrict__ absmax_v, int zero_grad,
+                                                                   const __nv_bfloat16* __restrict__ g16, float* __restrict__ ema,
+                                                                   const int64_t* __restrict__ step, float ema_decay) {
+    adamw8bit_chunks_body<true>(p, g, shadow, n_shadow, chunks, n_chunks, hp, qmaps, m32, v32, qm, qv, absmax_m, absmax_v, zero_grad, g16,
+                                ema, step, ema_decay);
+}
+
+// Exchanges p and the EMA over (arena offset, length, EMA offset) rows and rewrites the bf16 shadow of the rows below n_shadow
+// from the new p, rounded as the update kernels round it: a second call restores p, the EMA and the shadow bit for bit.
+__global__ void __launch_bounds__(256) ema_swap_chunks_kernel(float* __restrict__ p, float* __restrict__ ema, __nv_bfloat16* __restrict__ shadow,
+                                                              int64_t n_shadow, const int64_t* __restrict__ rows, int n_rows) {
+    pdl_sync();
+    for (int c = blockIdx.x; c < n_rows; c += gridDim.x) {
+        const int64_t off = rows[3 * c], len = rows[3 * c + 1], eoff = rows[3 * c + 2];
+        const bool sh = shadow != nullptr && off < n_shadow;
+        float4* p4 = reinterpret_cast<float4*>(p + off);
+        float4* e4 = reinterpret_cast<float4*>(ema + eoff);
+        uint2* s2 = reinterpret_cast<uint2*>(shadow + off);
+        const int nv = int(len >> 2);
+        for (int i = threadIdx.x; i < nv; i += blockDim.x) {
+            const float4 pp = p4[i], ee = e4[i];
+            p4[i] = ee;
+            e4[i] = pp;
+            if (sh) s2[i] = make_uint2(pack_bf16(ee.x, ee.y), pack_bf16(ee.z, ee.w));
         }
     }
 }
@@ -342,6 +446,53 @@ int t2v_adamw8bit_chunks(float* p, float* g, const void* g_bf16, void* shadow_bf
                                   static_cast<uint8_t*>(code_m), static_cast<uint8_t*>(code_v), absmax_m, absmax_v, int(zero_grad),
                                   static_cast<const __nv_bfloat16*>(g_bf16)));
     return launch_checked(rc, "adamw8bit_chunks");
+}
+
+static int check_ema(const float* ema, const int64_t* step, float ema_decay, const char* who) {
+    if (!ema || !step) return fail(-2, "%s: ema and step must not be NULL", who);
+    if (reinterpret_cast<uintptr_t>(ema) & 15u) return fail(-2, "%s: ema must be 16-byte aligned", who);
+    if (!(ema_decay >= 0.f && ema_decay <= 1.f)) return fail(-2, "%s: ema_decay must lie in [0, 1]", who);
+    return 0;
+}
+
+int t2v_adamw_ema_chunks(float* p, float* g, const void* g_bf16, float* m, float* v, void* shadow_bf16, int64_t n_shadow, const int64_t* chunks,
+                         int32_t n_chunks, const float* hp, int32_t zero_grad, float* ema, const int64_t* step, float ema_decay, void* stream) {
+    if (n_chunks <= 0) return 0;
+    if ((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(m) | reinterpret_cast<uintptr_t>(v)) & 15u)
+        return fail(-2, "adamw_ema_chunks: p, g, m, v must be 16-byte aligned");
+    if (shadow_bf16 && (reinterpret_cast<uintptr_t>(shadow_bf16) & 7u)) return fail(-2, "adamw_ema_chunks: shadow must be 8-byte aligned");
+    if (const int rc = check_ema(ema, step, ema_decay, "adamw_ema_chunks")) return rc;
+    const int rc = int(launch_pdl(adamw_ema_chunks_kernel, dim3(chunk_grid(n_chunks)), dim3(256), size_t(0), static_cast<cudaStream_t>(stream), p, g,
+                                  m, v, static_cast<__nv_bfloat16*>(shadow_bf16), n_shadow, chunks, int(n_chunks), hp, int(zero_grad),
+                                  static_cast<const __nv_bfloat16*>(g_bf16), ema, step, ema_decay));
+    return launch_checked(rc, "adamw_ema_chunks");
+}
+
+int t2v_adamw8bit_ema_chunks(float* p, float* g, const void* g_bf16, void* shadow_bf16, int64_t n_shadow, const int64_t* chunks, int32_t n_chunks,
+                             const float* hp, const float* qmaps, float* m32, float* v32, void* code_m, void* code_v, float* absmax_m,
+                             float* absmax_v, int32_t zero_grad, float* ema, const int64_t* step, float ema_decay, void* stream) {
+    if (n_chunks <= 0) return 0;
+    if ((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(m32) | reinterpret_cast<uintptr_t>(v32)) &
+        15u)
+        return fail(-2, "adamw8bit_ema_chunks: p, g, m32, v32 must be 16-byte aligned");
+    if ((reinterpret_cast<uintptr_t>(code_m) | reinterpret_cast<uintptr_t>(code_v)) & 3u)
+        return fail(-2, "adamw8bit_ema_chunks: code_m, code_v must be 4-byte aligned");
+    if (shadow_bf16 && (reinterpret_cast<uintptr_t>(shadow_bf16) & 7u)) return fail(-2, "adamw8bit_ema_chunks: shadow must be 8-byte aligned");
+    if (const int rc = check_ema(ema, step, ema_decay, "adamw8bit_ema_chunks")) return rc;
+    const int rc = int(launch_pdl(adamw8bit_ema_chunks_kernel, dim3(chunk_grid(n_chunks)), dim3(256), size_t(0), static_cast<cudaStream_t>(stream),
+                                  p, g, static_cast<__nv_bfloat16*>(shadow_bf16), n_shadow, chunks, int(n_chunks), hp, qmaps, m32, v32,
+                                  static_cast<uint8_t*>(code_m), static_cast<uint8_t*>(code_v), absmax_m, absmax_v, int(zero_grad),
+                                  static_cast<const __nv_bfloat16*>(g_bf16), ema, step, ema_decay));
+    return launch_checked(rc, "adamw8bit_ema_chunks");
+}
+
+int t2v_ema_swap_chunks(float* p, float* ema, void* shadow_bf16, int64_t n_shadow, const int64_t* rows, int32_t n_rows, void* stream) {
+    if (n_rows <= 0) return 0;
+    if ((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(ema)) & 15u) return fail(-2, "ema_swap_chunks: p, ema must be 16-byte aligned");
+    if (shadow_bf16 && (reinterpret_cast<uintptr_t>(shadow_bf16) & 7u)) return fail(-2, "ema_swap_chunks: shadow must be 8-byte aligned");
+    const int rc = int(launch_pdl(ema_swap_chunks_kernel, dim3(chunk_grid(n_rows)), dim3(256), size_t(0), static_cast<cudaStream_t>(stream), p, ema,
+                                  static_cast<__nv_bfloat16*>(shadow_bf16), n_shadow, rows, int(n_rows)));
+    return launch_checked(rc, "ema_swap_chunks");
 }
 
 int t2v_counter_add(int64_t* counter, int64_t value, void* stream) {

@@ -11,7 +11,14 @@ Frozen parameters are never touched (torch semantics: grad None => skipped, no w
 
 `AdamW8bit` (`use_8bit_adam`, reference train.py:238-249) is the same step with blockwise 8-bit moments for tensors of at
 least 4096 elements; its algorithm is stated on the class and on `dynamic_map`.
+
+With `ema_decay` (`use_ema`), both keep an exponential moving average of the trained weights, updated by the same kernel
+launch as the weights (diffusers' `EMAModel` with its default arguments; see `FusedAdamW`).
 """
+import bisect
+import contextlib
+import math
+
 import torch
 
 from . import prims
@@ -20,8 +27,24 @@ from .runtime import _align
 CHUNK = 1 << 16   # elements per chunk-table entry
 
 
+def check_ema_decay(ema_decay):
+    """The EMA decay cap as a float; ValueError unless it is finite and in [0, 1]."""
+    d = float(ema_decay)
+    if not (math.isfinite(d) and 0.0 <= d <= 1.0):
+        raise ValueError(f"ema_decay = {ema_decay!r}: the EMA decay must be a finite number in [0, 1]")
+    return d
+
+
 class FusedAdamW(torch.optim.Optimizer):
-    def __init__(self, arena, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-2, max_grad_norm=None):
+    """ema_decay (None: no EMA): keep an fp32 exponential moving average of every trainable tensor, updated in the update
+    kernel on the new weights while they are still in registers.  With k the step count after this step's increment,
+    d_1 = 0 and d_k = min(ema_decay, k / (9 + k)), and ema -= (1 - d_k) * (ema - p): diffusers' `EMAModel.step` with its
+    defaults (`(1 + s) / (10 + s)` with s = k - 1, no warm-up power, `min_decay` 0, `update_after_step` 0).  k is read on
+    the device, so a replayed CUDA graph uses each step's decay.  The EMA is compact (the trainable tensors of this
+    optimizer only, in arena order, each starting at a multiple of 64 elements) and starts as a copy of the weights; a frozen
+    parameter's EMA is the parameter itself.  `ema_weights()` swaps it into the model."""
+
+    def __init__(self, arena, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-2, max_grad_norm=None, ema_decay=None):
         super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay))
         self.arena = arena
         self.max_grad_norm = max_grad_norm
@@ -34,6 +57,8 @@ class FusedAdamW(torch.optim.Optimizer):
                 if id(p) not in self._off:
                     raise ValueError("FusedAdamW only drives parameters that live in the arena")
         self._alloc_state()
+        self.ema_decay = None if ema_decay is None else check_ema_decay(ema_decay)
+        self.ema = None if ema_decay is None else self._alloc_ema()
         self._sets = None
         self._build()
 
@@ -45,9 +70,52 @@ class FusedAdamW(torch.optim.Optimizer):
         """Name -> device tensor of the optimizer's moment state (what `state_dict` saves besides the step count)."""
         return {"exp_avg": self.exp_avg, "exp_avg_sq": self.exp_avg_sq}
 
+    def _saved(self):
+        """_moments() plus the EMA when there is one: every tensor `state_dict` saves besides the step count."""
+        return self._moments() if self.ema is None else dict(self._moments(), ema=self.ema)
+
     def state_tensors(self):
         """Every device tensor one step mutates besides the weights and gradients (a CUDA-graph capture snapshots them)."""
-        return list(self._moments().values()) + [self.state_dev, self.sq]
+        return list(self._saved().values()) + [self.state_dev, self.sq]
+
+    # ------------------------------------------------------------------------------------------------ EMA
+    def _trainable_sorted(self):
+        return sorted((p for g in self.param_groups for p in g["params"] if p.requires_grad), key=lambda q: self._off[id(q)])
+
+    def _alloc_ema(self):
+        """The compact EMA, a copy of the current trainable weights (alignment padding included, which the arena keeps at 0)."""
+        master = self.arena.master
+        self._ema_starts, self._ema_base, n = [], [], 0   # arena offset and EMA offset of each trainable tensor, arena order
+        for p in self._trainable_sorted():
+            self._ema_starts.append(self._off[id(p)])
+            self._ema_base.append(n)
+            n += _align(p.numel())
+        ema = torch.empty(n, device=master.device, dtype=torch.float32)
+        for a, e, b in zip(self._ema_starts, self._ema_base, self._ema_base[1:] + [n]):
+            ema[e:b].copy_(master[a:a + b - e])
+        return ema
+
+    def _ema_rows(self, rows):
+        """`rows` with the EMA offset of each row's first element appended.  A row spans arena-adjacent trainable tensors
+        only, and those are adjacent in the EMA as well."""
+        out = []
+        for r in rows:
+            i = bisect.bisect_right(self._ema_starts, r[0]) - 1
+            out.append(tuple(r) + (self._ema_base[i] + r[0] - self._ema_starts[i],))
+        return out
+
+    @contextlib.contextmanager
+    def ema_weights(self):
+        """Within the `with` block the model holds the EMA weights (master and bf16 shadow); on exit the training weights
+        and the EMA are swapped back, bit for bit.  Frozen parameters are left as they are."""
+        if self.ema is None:
+            raise RuntimeError("ema_weights() needs an optimizer built with ema_decay")
+        ar = self.arena
+        prims.ema_swap_chunks(ar.master, self.ema, ar.shadow, ar.n_mat, self._ema_swap)
+        try:
+            yield
+        finally:
+            prims.ema_swap_chunks(ar.master, self.ema, ar.shadow, ar.n_mat, self._ema_swap)
 
     # ------------------------------------------------------------------------------------------------ chunk tables
     @staticmethod
@@ -94,8 +162,12 @@ class FusedAdamW(torch.optim.Optimizer):
             table = torch.tensor(chunks, dtype=torch.int64, device=dev).contiguous()
             sets.append({"groups": gis, "key": key, "chunks": table, "norm_chunks": table[:, :2].contiguous() if table.shape[1] > 2 else table,
                          "n": sum(c[1] for c in chunks)})
+            if self.ema is not None:
+                sets[-1]["ema_chunks"] = torch.tensor(self._ema_rows(chunks), dtype=torch.int64, device=dev)
         if not sets:
             raise ValueError("FusedAdamW: no trainable parameters")
+        if self.ema is not None:   # (arena offset, length, EMA offset) over every set: the rows ema_weights() swaps
+            self._ema_swap = torch.cat([s["ema_chunks"][:, [0, 1, -1]] for s in sets]).contiguous()
         self._sets = sets
         self.hp_host = torch.zeros((len(sets), 5), dtype=torch.float32)
         if dev.type == "cuda":
@@ -142,7 +214,11 @@ class FusedAdamW(torch.optim.Optimizer):
 
     def _update(self, s, hp_row, zero_grad, grad_bf16):
         ar = self.arena
-        prims.adamw_chunks(ar.master, ar.grad, self.exp_avg, self.exp_avg_sq, ar.shadow, ar.n_mat, s["chunks"], hp_row, zero_grad, grad_bf16)
+        if self.ema is None:
+            prims.adamw_chunks(ar.master, ar.grad, self.exp_avg, self.exp_avg_sq, ar.shadow, ar.n_mat, s["chunks"], hp_row, zero_grad, grad_bf16)
+        else:
+            prims.adamw_ema_chunks(ar.master, ar.grad, self.exp_avg, self.exp_avg_sq, ar.shadow, ar.n_mat, s["ema_chunks"], hp_row, self.ema,
+                                   self.state_dev, self.ema_decay, zero_grad, grad_bf16)
 
     @torch.no_grad()
     def step(self, closure=None, zero_grad=True):
@@ -166,14 +242,14 @@ class FusedAdamW(torch.optim.Optimizer):
     # ------------------------------------------------------------------------------------------------ checkpointing
     def state_dict(self):
         d = super().state_dict()
-        d["fused"] = dict(self._moments(), step=self.steps)
+        d["fused"] = dict(self._saved(), step=self.steps)
         return d
 
     def load_state_dict(self, state_dict):
         fused = state_dict.pop("fused", None)
         super().load_state_dict(state_dict)
         if fused is not None:
-            for name, t in self._moments().items():
+            for name, t in self._saved().items():
                 t.copy_(fused[name])
             self.state_dev.fill_(int(fused["step"]))
 
@@ -260,5 +336,10 @@ class AdamW8bit(FusedAdamW):
 
     def _update(self, s, hp_row, zero_grad, grad_bf16):
         ar = self.arena
-        prims.adamw8bit_chunks(ar.master, ar.grad, ar.shadow, ar.n_mat, s["chunks"], hp_row, self.qmaps, self.exp_avg32, self.exp_avg_sq32,
-                               self.code_m, self.code_v, self.absmax_m, self.absmax_v, zero_grad, grad_bf16)
+        if self.ema is None:
+            prims.adamw8bit_chunks(ar.master, ar.grad, ar.shadow, ar.n_mat, s["chunks"], hp_row, self.qmaps, self.exp_avg32, self.exp_avg_sq32,
+                                   self.code_m, self.code_v, self.absmax_m, self.absmax_v, zero_grad, grad_bf16)
+        else:
+            prims.adamw8bit_ema_chunks(ar.master, ar.grad, ar.shadow, ar.n_mat, s["ema_chunks"], hp_row, self.qmaps, self.exp_avg32,
+                                       self.exp_avg_sq32, self.code_m, self.code_v, self.absmax_m, self.absmax_v, self.ema, self.state_dev,
+                                       self.ema_decay, zero_grad, grad_bf16)

@@ -362,6 +362,44 @@ def adamw8bit_chunks(p, g, shadow, n_shadow, chunks, hp_row, qmaps, m32, v32, co
                                                    _p(absmax_v), int(bool(zero_grad)), _stream()))
 
 
+def _chk_ema(ema, step, chunks, cols):
+    _chk_f32(ema)
+    assert ema is not None and step.dtype == torch.int64 and step.is_cuda
+    assert chunks.dtype == torch.int64 and chunks.dim() == 2 and chunks.shape[1] == cols and chunks.is_contiguous()
+
+
+def adamw_ema_chunks(p, g, m, v, shadow, n_shadow, chunks, hp_row, ema, step, ema_decay, zero_grad=True, g_bf16=None):
+    """adamw_chunks over (arena offset, length, EMA offset) rows, then the EMA of each updated element: with k = step[0]
+    (device int64, read when the kernel runs), ema -= (1 - d_k) * (ema - p), d_1 = 0, d_k = min(ema_decay, k / (9 + k))."""
+    _chk_f32(p, g, m, v, hp_row)
+    _chk_bf16(shadow, g_bf16)
+    _chk_ema(ema, step, chunks, 3)
+    native.check(native.lib().t2v_adamw_ema_chunks(_p(p), _p(g), _p(g_bf16), _p(m), _p(v), _p(shadow), int(n_shadow), _p(chunks),
+                                                   chunks.shape[0], _p(hp_row), int(bool(zero_grad)), _p(ema), _p(step), float(ema_decay),
+                                                   _stream()))
+
+
+def adamw8bit_ema_chunks(p, g, shadow, n_shadow, chunks, hp_row, qmaps, m32, v32, code_m, code_v, absmax_m, absmax_v, ema, step, ema_decay,
+                         zero_grad=True, g_bf16=None):
+    """adamw8bit_chunks over (arena offset, length, state offset, bits, EMA offset) rows plus the EMA of adamw_ema_chunks."""
+    _chk_f32(p, g, hp_row, qmaps, m32, v32, absmax_m, absmax_v)
+    _chk_bf16(shadow, g_bf16)
+    _chk_ema(ema, step, chunks, 5)
+    assert code_m.dtype == code_v.dtype == torch.uint8 and code_m.is_cuda and code_v.is_cuda and qmaps.numel() == 512
+    native.check(native.lib().t2v_adamw8bit_ema_chunks(_p(p), _p(g), _p(g_bf16), _p(shadow), int(n_shadow), _p(chunks), chunks.shape[0],
+                                                       _p(hp_row), _p(qmaps), _p(m32), _p(v32), _p(code_m), _p(code_v), _p(absmax_m),
+                                                       _p(absmax_v), int(bool(zero_grad)), _p(ema), _p(step), float(ema_decay), _stream()))
+
+
+def ema_swap_chunks(p, ema, shadow, n_shadow, rows):
+    """Exchange p and ema over the (arena offset, length, EMA offset) rows and rewrite the bf16 shadow of the rows below
+    n_shadow from the new p; a second call restores all three bit for bit."""
+    _chk_f32(p, ema)
+    _chk_bf16(shadow)
+    assert rows.dtype == torch.int64 and rows.dim() == 2 and rows.shape[1] == 3 and rows.is_contiguous()
+    native.check(native.lib().t2v_ema_swap_chunks(_p(p), _p(ema), _p(shadow), int(n_shadow), _p(rows), rows.shape[0], _stream()))
+
+
 def scale_cast_f32_bf16(src, dst, alpha):
     """dst (bf16) = alpha * src (fp32): gradient compression before the data-parallel all-reduce."""
     _chk_f32(src)

@@ -18,6 +18,7 @@ is a full pipeline - the complete pipeline directory (`save_pipe`, train.py:395-
 `validation_steps` (sampling.py: DPM-Solver++ preview with the trained UNet in eval mode, train.py:908-958).
 """
 import argparse
+import contextlib
 import itertools
 import math
 import os
@@ -208,6 +209,8 @@ def main(
     resume_step: Optional[int] = None,
     mixed_precision: Optional[str] = "fp16",
     use_8bit_adam: bool = False,
+    use_ema: bool = False,
+    ema_decay: float = 0.9999,
     enable_xformers_memory_efficient_attention: bool = True,
     enable_torch_2_attn: bool = False,
     seed: Optional[int] = None,
@@ -248,6 +251,11 @@ def main(
     fused_adamw = bool(kwargs.get("fused_adamw", True))   # optim.FusedAdamW on the flat arena (SURVEY 8(f) row 1); False: torch AdamW
     if use_8bit_adam and not fused_adamw:
         raise ValueError("use_8bit_adam runs optim.AdamW8bit on the flat arena; it cannot be combined with fused_adamw=False")
+    if use_ema:   # the EMA is updated inside the fused optimizer step (optim.FusedAdamW ema_decay)
+        if not fused_adamw:
+            raise ValueError("use_ema keeps the EMA inside the fused optimizer step; it cannot be combined with fused_adamw=False")
+        from .optim import check_ema_decay
+        check_ema_decay(ema_decay)
     # noise schedule and loss target of the checkpoint (train.py:119, 792-800); an unsupported config fails here, before any
     # weights move.  `rescale_schedule` stays a no-op: in the reference it never reaches add_noise (SURVEY H5).
     abar, prediction_type = load_noise_schedule(pretrained_model_path)
@@ -302,7 +310,7 @@ def main(
         from .optim import AdamW8bit, FusedAdamW
         cls = AdamW8bit if use_8bit_adam else FusedAdamW
         optimizer = cls(stepper.arena, groups, lr=learning_rate, betas=(adam_beta1, adam_beta2), weight_decay=adam_weight_decay,
-                        eps=adam_epsilon, max_grad_norm=max_grad_norm)
+                        eps=adam_epsilon, max_grad_norm=max_grad_norm, ema_decay=ema_decay if use_ema else None)
         stepper.attach_optimizer(optimizer)   # the update (clip + AdamW + shadow refresh + grad zeroing) is part of the step graph
     else:
         optimizer = torch.optim.AdamW(groups, lr=learning_rate, betas=(adam_beta1, adam_beta2), weight_decay=adam_weight_decay,
@@ -403,20 +411,21 @@ def main(
                 print(f"step {global_step}/{max_train_steps} loss {loss.item():.5f} ({(time.time() - t0) / global_step:.3f} s/step)")
             if rank == 0 and global_step % checkpointing_steps == 0:
                 save_checkpoint(unet, lora_manager, output_dir, global_step, use_unet_lora, save_pretrained_model,
-                                pretrained_model_path=pretrained_model_path)
+                                pretrained_model_path=pretrained_model_path, ema=optimizer if use_ema else None)
             if rank == 0 and validation_data and validation_steps and global_step % validation_steps == 0 and vae is not None \
                     and text_encoder is not None and tokenizer is not None and getattr(vae, "decoder", None) is not None:
                 from .sampling import validation_sample
-                validation_sample(unet, vae, text_encoder, tokenizer, validation_data, os.path.join(output_dir, "samples"), global_step,
-                                  batch.get("text_prompt", [""])[0] if isinstance(batch.get("text_prompt"), (list, tuple)) else "", dev,
-                                  alphas_cumprod=abar, prediction_type=prediction_type)
+                with optimizer.ema_weights() if use_ema else contextlib.nullcontext():   # preview what a user would export
+                    validation_sample(unet, vae, text_encoder, tokenizer, validation_data, os.path.join(output_dir, "samples"), global_step,
+                                      batch.get("text_prompt", [""])[0] if isinstance(batch.get("text_prompt"), (list, tuple)) else "",
+                                      dev, alphas_cumprod=abar, prediction_type=prediction_type)
             if global_step >= max_train_steps:
                 break
     if world > 1:
         dist.barrier()
     if rank == 0:
         save_checkpoint(unet, lora_manager, output_dir, global_step, use_unet_lora, save_pretrained_model, final=True,
-                        pretrained_model_path=pretrained_model_path)
+                        pretrained_model_path=pretrained_model_path, ema=optimizer if use_ema else None)
     return {"steps": global_step, "step_times": step_times, "stepper": stepper, "optimizer": optimizer}
 
 
@@ -448,8 +457,11 @@ def save_pipe(pretrained_model_path, unet, path):
     return copied
 
 
-def save_checkpoint(unet, lora_manager, output_dir, step, use_unet_lora, save_pretrained_model, final=False, pretrained_model_path=None):
-    """LoRA in the cloneofsimo list format (`lora/<step>_unet.pt`) and, with save_pretrained_model, the pipeline directory."""
+def save_checkpoint(unet, lora_manager, output_dir, step, use_unet_lora, save_pretrained_model, final=False, pretrained_model_path=None,
+                    ema=None):
+    """LoRA in the cloneofsimo list format (`lora/<step>_unet.pt`) and, with save_pretrained_model, the pipeline directory.
+    ema (`use_ema`): the optimizer holding the EMA of the weights; the EMA weights are then written as well, as
+    `lora/<step>_unet_ema.pt` and (save_pretrained_model) `unet_ema/` in the diffusers UNet layout."""
     path = output_dir if final else os.path.join(output_dir, f"checkpoint-{step}")
     os.makedirs(path, exist_ok=True)
     if use_unet_lora:   # the reference saves the LoRA files and (save_pretrained_model) the pipeline: train.py:908-958
@@ -461,6 +473,12 @@ def save_checkpoint(unet, lora_manager, output_dir, step, use_unet_lora, save_pr
             save_pipe(pretrained_model_path, unet, path)
         else:
             unet.save_pretrained(os.path.join(path, "unet"))
+    if ema is not None:
+        with ema.ema_weights():
+            if use_unet_lora:
+                save_lora_weight(unet, os.path.join(path, "lora", f"{step}_unet_ema.pt"), lora_manager.unet_replace_modules)
+            if save_pretrained_model:
+                unet.save_pretrained(os.path.join(path, "unet_ema"))
 
 
 def load_config(path):

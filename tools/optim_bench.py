@@ -1,10 +1,11 @@
 #!/usr/bin/env python
-"""Optimizer cost of blockwise 8-bit AdamW (optim.AdamW8bit) next to fp32 AdamW (optim.FusedAdamW) on an H100.
+"""Optimizer cost of blockwise 8-bit AdamW (optim.AdamW8bit) next to fp32 AdamW (optim.FusedAdamW), each with and without the
+weight EMA (`ema_decay`, `use_ema`), on an H100.
 
 cfg 2 (the ms-1.7b UNet as bench.py builds it, all 1.41 B parameters trainable, random gradient):
   * launch() time of each optimizer (global-norm clip + update), CUDA events, the two alternated and each timed twice;
   * algorithmic bytes per trainable parameter and the achieved TB/s against the 3.35 TB/s data-sheet HBM3 bandwidth;
-  * optimizer-state bytes, from torch.cuda.memory_allocated before and after constructing the optimizer;
+  * optimizer-state bytes, from torch.cuda.memory_allocated before and after constructing the optimizer, and the EMA's share;
   * the cfg-2 step (CUDA-graph replay, --steps timed after --warmup) with each optimizer attached, alternated, each twice.
 LoRA workload (bench.py --workload lora): the state and launch() lines, and how much of the state saving comes from covering
 only the trainable tensors (a compact fp32 state, computed) and how much from 8 bits.
@@ -27,7 +28,9 @@ from t2v_b200.optim import AdamW8bit, FusedAdamW  # noqa: E402
 from t2v_b200.runtime import ParamArena, _align  # noqa: E402
 
 HBM_TBS = 3.35   # H100 SXM data sheet
-OPTIMIZERS = (("fused_adamw", FusedAdamW), ("adamw8bit", AdamW8bit))
+EMA_DECAY = 0.9999
+OPTIMIZERS = (("fused_adamw", FusedAdamW, None), ("fused_adamw_ema", FusedAdamW, EMA_DECAY), ("adamw8bit", AdamW8bit, None),
+              ("adamw8bit_ema", AdamW8bit, EMA_DECAY))
 
 
 def gpu_info():
@@ -36,23 +39,23 @@ def gpu_info():
     return {"device": torch.cuda.get_device_name(0), "nvidia_smi name, power.limit, clocks.max.sm": q.stdout.strip() or q.stderr.strip()}
 
 
-def make(cls, arena, params):
+def make(cls, arena, params, ema_decay):
     torch.cuda.synchronize()
     before = torch.cuda.memory_allocated()
-    opt = cls(arena, [dict(params=params)], lr=5e-6, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-2, max_grad_norm=1.0)
+    opt = cls(arena, [dict(params=params)], lr=5e-6, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-2, max_grad_norm=1.0, ema_decay=ema_decay)
     torch.cuda.synchronize()
     return opt, torch.cuda.memory_allocated() - before
 
 
 def algorithmic_bytes(opt):
     """Bytes one launch() moves: 4 (gradient read of the norm) + 34 per fp32-state element; 4 + 22 per 8-bit element plus
-    16 per 256-element block (absmax of m and v, read and written)."""
+    16 per 256-element block (absmax of m and v, read and written); 8 more per element with an EMA (its read and write)."""
     total = 0
     for s in opt._sets:
         for row in s["chunks"].tolist():
             n = row[1]
             total += 26 * n + 16 * ((n + 255) // 256) if len(row) == 4 and row[3] == 8 else 38 * n
-    return total
+    return total + (8 * opt.ema.numel() if opt.ema is not None else 0)
 
 
 def time_launch(opt, arena, n):
@@ -67,15 +70,16 @@ def time_launch(opt, arena, n):
 
 def optimizer_leg(arena, params, reps, n):
     opts, out = {}, {}
-    for name, cls in OPTIMIZERS:
-        opts[name], mem = make(cls, arena, params)
+    for name, cls, ema_decay in OPTIMIZERS:
+        opts[name], mem = make(cls, arena, params, ema_decay)
         out[name] = {"state_bytes_allocated": mem, "trainable_elements": opts[name].trainable_elements,
-                     "algorithmic_bytes": algorithmic_bytes(opts[name]), "launch_ms": []}
+                     "algorithmic_bytes": algorithmic_bytes(opts[name]), "launch_ms": [],
+                     "ema_bytes": 4 * opts[name].ema.numel() if ema_decay is not None else 0}
         out[name]["bytes_per_param"] = out[name]["algorithmic_bytes"] / out[name]["trainable_elements"]
     for _ in range(reps):
-        for name, _ in OPTIMIZERS:
+        for name, _, _ in OPTIMIZERS:
             out[name]["launch_ms"].append(time_launch(opts[name], arena, n))
-    for name, _ in OPTIMIZERS:
+    for name, _, _ in OPTIMIZERS:
         best = min(out[name]["launch_ms"])
         out[name]["achieved_tbs"] = out[name]["algorithmic_bytes"] / (best / 1e3) / 1e12
         out[name]["frac_of_hbm_peak"] = out[name]["achieved_tbs"] / HBM_TBS
@@ -102,10 +106,10 @@ def main():
     gc.collect()
     torch.cuda.empty_cache()
     devin = [x.to(dev) for x in bench.synthetic_inputs(1, bench.CFG2, 1234)]
-    step_ms = {name: [] for name, _ in OPTIMIZERS}
+    step_ms = {name: [] for name, _, _ in OPTIMIZERS}
     for _ in range(args.reps):
-        for name, cls in OPTIMIZERS:
-            opt, _ = make(cls, step.arena, trainable)
+        for name, cls, ema_decay in OPTIMIZERS:
+            opt, _ = make(cls, step.arena, trainable, ema_decay)
             step.attach_optimizer(opt)
             for _ in range(args.warmup):
                 step(*devin)
@@ -115,7 +119,7 @@ def main():
             del opt
             gc.collect()
             torch.cuda.empty_cache()
-    for name, _ in OPTIMIZERS:
+    for name, _, _ in OPTIMIZERS:
         report["cfg2"][name]["step_ms"] = step_ms[name]
     report["cfg2"]["step"] = f"cfg-2 step (one fwd+bwd pass + optimizer, CUDA-graph replay), {args.steps} steps after {args.warmup} warm-up"
     del step, unet, trainable, devin
