@@ -343,6 +343,19 @@ int t2v_adamw8bit_ema_chunks(float* p, float* g, const void* g_bf16, void* shado
                              float* absmax_v, int32_t zero_grad, float* ema, const int64_t* step, float ema_decay, void* stream);
 int t2v_ema_swap_chunks(float* p, float* ema, void* shadow_bf16, int64_t n_shadow, const int64_t* rows, int32_t n_rows, void* stream);
 
+/* Stable (loralib-style) LoRA on a convolution: W_eff = W + scaling * view(B @ A), A [r*k][Cin*k], B [Cout*k][r*k] fp32
+ * row-major (stable_lora/lora.py Conv2d / Conv3d forward).  With f = ((o*Cin + c)*k + kh)*k + kw the logical (o, c, kh, kw)
+ * element of the Conv2d view is BA[f / (Cin*k)][f % (Cin*k)]; the Conv3d (3,1,1) view (k = 3) is the mean of the three
+ * consecutive BA columns f = ((o*Cin + c)*3 + t)*3 + 0..2.  Weights are in the physical layout [Cout][KH][KW][Cin] ([Cout][3][1][Cin]).
+ *   t2v_lora_delta_merge  out_bf16 = bf16(base + scaling * view(B @ A)): the fp32 base is added before the single rounding.
+ *   t2v_lora_delta_grad   dBA = scaling * view^T(dw) (Conv3d: dw / 3 on each averaged column), then dB += dBA A^T and
+ *                         dA += B^T dBA (fp32, red.add, so not bitwise reproducible); dw is read once.
+ * k must be 1 or 3 (Conv2d) or 3 (conv3d != 0); 1 <= r <= 256.                                                             */
+int t2v_lora_delta_merge(const float* base, const float* A, const float* B, float scaling, int32_t k, int32_t conv3d, int32_t cout,
+                         int32_t cin, int32_t r, void* out_bf16, void* stream);
+int t2v_lora_delta_grad(const float* dw, const float* A, const float* B, float scaling, int32_t k, int32_t conv3d, int32_t cout,
+                        int32_t cin, int32_t r, float* dA, float* dB, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

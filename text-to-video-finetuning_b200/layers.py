@@ -35,13 +35,20 @@ def _is_lora(m):
     return hasattr(m, "lora_down") and hasattr(m, "lora_up")
 
 
+def _is_stable_lora(m):
+    return hasattr(m, "lora_A") and hasattr(m, "lora_B")
+
+
 def _lora_base(m):
     return m.linear if hasattr(m, "linear") else m.conv
 
 
 def run_linear(m, x, residual=None, out_fp32=False, stats_rows=0):
-    """Apply an nn.Linear (or a cloneofsimo-style LoRA wrapper around one) to a token matrix.  stats_rows > 0: the output
+    """Apply an nn.Linear (or a cloneofsimo / stable LoRA wrapper around one) to a token matrix.  stats_rows > 0: the output
     feeds a GroupNorm - let the GEMM epilogue produce its per-frame channel sums (stats_rows = tokens per frame)."""
+    if _is_stable_lora(m):
+        from .utils.stable_lora import stable_linear_forward
+        return stable_linear_forward(m, x, residual, out_fp32, stats_rows)
     if _is_lora(m):
         from .utils.lora import lora_linear_forward
         return lora_linear_forward(m, x, residual, out_fp32, stats_rows)
@@ -50,6 +57,9 @@ def run_linear(m, x, residual=None, out_fp32=False, stats_rows=0):
 
 def run_conv(m, x, rowbias=None, residual=None, stride=1, pads=(1, 1, 1, 1), rb_div=1, cin_pad=0, cout_pad=0, stats_rows=0):
     """Apply an nn.Conv2d / nn.Conv3d((3,1,1)) (or its LoRA wrapper) to a channels-last batch (stats_rows: see run_linear)."""
+    if _is_stable_lora(m):
+        from .utils.stable_lora import stable_conv_forward
+        return stable_conv_forward(m, x, rowbias, residual, stride, pads, rb_div, cin_pad, cout_pad, stats_rows)
     if _is_lora(m):
         from .utils.lora import lora_conv_forward
         return lora_conv_forward(m, x, rowbias, residual, stride, pads, rb_div, cin_pad, cout_pad, stats_rows)

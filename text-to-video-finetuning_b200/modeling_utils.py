@@ -81,12 +81,13 @@ class ModelMixin(torch.nn.Module):
             model = model.to(torch_dtype)
         return model.eval()
 
-    def save_pretrained(self, save_directory, safe_serialization=True, **unused):
+    def save_pretrained(self, save_directory, safe_serialization=True, state_dict=None, **unused):
+        """state_dict: written instead of self.state_dict() (as in diffusers)."""
         os.makedirs(save_directory, exist_ok=True)
         cfg = {k: (list(v) if isinstance(v, tuple) else v) for k, v in self.config.items()}
         with open(os.path.join(save_directory, self.config_name), "w") as f:
             json.dump(cfg, f, indent=2)
-        sd = {k: v.detach().cpu().contiguous() for k, v in self.state_dict().items()}
+        sd = {k: v.detach().cpu().contiguous() for k, v in (self.state_dict() if state_dict is None else state_dict).items()}
         if safe_serialization:
             from safetensors.torch import save_file
             save_file(sd, os.path.join(save_directory, self.weights_name + ".safetensors"))

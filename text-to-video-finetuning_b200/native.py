@@ -81,6 +81,7 @@ EXPORTS = [
     "t2v_upsample_nearest_bwd", "t2v_copy_cols", "t2v_colsum", "t2v_colsum_f32", "t2v_softmax_fwd", "t2v_softmax_bwd",
     "t2v_timestep_embedding", "t2v_attn_small_fwd", "t2v_attn_small_bwd",
     "t2v_attn_long_fwd", "t2v_attn_long_bwd",
+    "t2v_lora_delta_merge", "t2v_lora_delta_grad",
 ]
 
 
@@ -152,6 +153,8 @@ def _declare(lib):
     lib.t2v_attn_small_bwd.argtypes = [vp] * 7 + [i64, i32, i64, i64, i64, i64, i64, i32, i32, i32, vp]
     lib.t2v_attn_long_fwd.argtypes = [vp] * 5 + [i64, i32, i64, i64, i64, i64, i64, i32, i32, i32, vp]
     lib.t2v_attn_long_bwd.argtypes = [vp] * 9 + [i64, i32, i64, i64, i64, i64, i64, i32, i32, i32, vp]
+    lib.t2v_lora_delta_merge.argtypes = [vp, vp, vp, f32] + [i32] * 5 + [vp, vp]
+    lib.t2v_lora_delta_grad.argtypes = [vp, vp, vp, f32] + [i32] * 5 + [vp, vp, vp]
     for name in EXPORTS:
         getattr(lib, name)  # every declared symbol must be exported
     return lib

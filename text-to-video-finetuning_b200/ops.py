@@ -48,11 +48,36 @@ class FusedWeight:
         return len(flags) == 1   # all trainable or all frozen
 
 
+class DeltaWeight:
+    """A frozen conv weight plus a stable-LoRA delta, W_eff = base + scaling * view(B @ A) (utils/stable_lora.py): `_Conv`
+    merges it into one bf16 weight (lora_delta.cu) and runs ONE GEMM with every epilogue of the plain conv; its backward
+    projects the weight gradient onto A and B.  conv3d: the (3,1,1) view, which averages triples of B @ A."""
+
+    def __init__(self, base, A, B, scaling, conv3d=False):
+        self.base, self.A, self.B, self.scaling, self.conv3d = base, A, B, float(scaling), bool(conv3d)
+
+    @property
+    def requires_grad(self):
+        return self.A.requires_grad or self.B.requires_grad
+
+    def merged_bf16(self):
+        return prims.lora_delta_merge(_cont(_phys(_f32(self.base))), _cont(_f32(self.A)), _cont(_f32(self.B)), self.scaling, self.conv3d)
+
+    def grad_scratch(self):
+        """Zeroed fp32 buffer in kernel layout for the gradient of W_eff (never the frozen base's own .grad)."""
+        return torch.zeros(_phys(self.base).shape, device=self.base.device, dtype=torch.float32)
+
+    def project_grad(self, dw, dA, dB):
+        prims.lora_delta_grad(dw, _cont(_f32(self.A)), _cont(_f32(self.B)), self.scaling, self.conv3d, dA, dB)
+
+
 def weight_bf16(p):
     """bf16 compute copy of a weight in kernel layout.  Uses the per-step flat shadow when the model has been
-    prepared by runtime.ParamArena, otherwise casts on the fly (our cast kernel)."""
+    prepared by runtime.ParamArena, otherwise casts on the fly (our cast kernel).  A DeltaWeight is merged here."""
     if isinstance(p, FusedWeight):
         return p.shadow
+    if isinstance(p, DeltaWeight):
+        return p.merged_bf16()
     sh = getattr(p, "_t2v_shadow", None)
     if sh is not None:
         return sh
@@ -266,7 +291,11 @@ class _Conv(Function):
             d_rowbias = d_rowbias_full[:, :Co - cout_pad].contiguous() if cout_pad else d_rowbias_full
         # parameter gradients (bias column sums, weight gradient) are leaves: they run on the side stream
         gb = grad_vec(bias) if (bias is not None and bias.requires_grad) else None
-        gw = grad_phys(weight) if weight.requires_grad else None
+        delta = isinstance(weight, DeltaWeight) and weight.requires_grad
+        if delta:   # the wgrad lands in a scratch of W_eff's shape, then is projected onto the LoRA factors
+            gw, gA, gB = weight.grad_scratch(), grad_vec(weight.A), grad_vec(weight.B)
+        else:
+            gw = grad_phys(weight) if weight.requires_grad else None
 
         def param_grads():
             # the plain bias gradient (column sums of dy) rides in the weight-gradient launch when both are wanted
@@ -287,9 +316,11 @@ class _Conv(Function):
                     gw.add_(tmp[:gw.shape[0], :, :, :gw.shape[3]])
                 else:
                     prims.conv_wgrad(x, dy, gw, stride, pads, dbias=gb if fuse_bias else None)
+                if delta:
+                    weight.project_grad(gw, gA, gB)
 
         if gb is not None or gw is not None:
-            _run_param_grads(param_grads, dy, x, d_rowbias_full)
+            _run_param_grads(param_grads, dy, x, d_rowbias_full, gw if delta else None)
         dx = None
         if ctx.needs_input_grad[0]:
             dx = prims.conv_dgrad(dy, w, (x.shape[1], x.shape[2]), stride, pads)
@@ -307,7 +338,8 @@ def conv(x, weight, bias=None, rowbias=None, residual=None, stride=1, pads=(1, 1
     """stats_rows > 0: also emit the per-(frame, channel) GroupNorm statistics of the output from the GEMM epilogue
     (stats_rows = output rows per frame); they ride on the returned tensor (see `carry`)."""
     holder = [] if stats_rows else None
-    y = _Conv.apply(x, weight, bias, rowbias, residual, stride, tuple(pads), rb_div, out_fp32, cin_pad, cout_pad, float(alpha), None,
+    anchor = weight.A if isinstance(weight, DeltaWeight) and weight.requires_grad else None
+    y = _Conv.apply(x, weight, bias, rowbias, residual, stride, tuple(pads), rb_div, out_fp32, cin_pad, cout_pad, float(alpha), anchor,
                     int(stats_rows), holder)
     return _with_stats(y, holder)
 

@@ -400,6 +400,37 @@ def ema_swap_chunks(p, ema, shadow, n_shadow, rows):
     native.check(native.lib().t2v_ema_swap_chunks(_p(p), _p(ema), _p(shadow), int(n_shadow), _p(rows), rows.shape[0], _stream()))
 
 
+def _delta_geom(w, A, B, conv3d):
+    """(Cout, Cin, k, r) of a stable-LoRA conv: w [Cout, KH, KW, Cin], A [r*k, Cin*k], B [Cout*k, r*k]."""
+    Co, KH, KW, Ci = w.shape
+    k = KH
+    assert (KH, KW) == ((3, 1) if conv3d else (k, k)), (w.shape, conv3d)
+    assert A.dim() == 2 and B.dim() == 2 and A.shape[1] == Ci * k and B.shape == (Co * k, A.shape[0]) and A.shape[0] % k == 0, \
+        (w.shape, A.shape, B.shape)
+    return Co, Ci, k, A.shape[0] // k
+
+
+def lora_delta_merge(base, A, B, scaling, conv3d):
+    """bf16 [Cout, KH, KW, Cin] = base + scaling * view(B @ A) for a stable-LoRA conv (include/t2v_b200.h); base is the fp32
+    weight in the same physical layout, A and B the fp32 LoRA factors."""
+    _chk_f32(base, A, B)
+    Co, Ci, k, r = _delta_geom(base, A, B, conv3d)
+    out = torch.empty(base.shape, device=base.device, dtype=torch.bfloat16)
+    native.check(native.lib().t2v_lora_delta_merge(_p(base), _p(A), _p(B), float(scaling), k, int(bool(conv3d)), Co, Ci, r, _p(out),
+                                                   _stream()))
+    return out
+
+
+def lora_delta_grad(dw, A, B, scaling, conv3d, dA, dB):
+    """dA += B^T dBA, dB += dBA A^T with dBA = scaling * view^T(dw): the gradient of a merged stable-LoRA conv weight (fp32
+    [Cout, KH, KW, Cin]) projected onto its factors."""
+    _chk_f32(dw, A, B, dA, dB)
+    assert dA.shape == A.shape and dB.shape == B.shape
+    Co, Ci, k, r = _delta_geom(dw, A, B, conv3d)
+    native.check(native.lib().t2v_lora_delta_grad(_p(dw), _p(A), _p(B), float(scaling), k, int(bool(conv3d)), Co, Ci, r, _p(dA), _p(dB),
+                                                  _stream()))
+
+
 def scale_cast_f32_bf16(src, dst, alpha):
     """dst (bf16) = alpha * src (fp32): gradient compression before the data-parallel all-reduce."""
     _chk_f32(src)

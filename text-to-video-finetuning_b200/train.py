@@ -1,7 +1,7 @@
 """`python train.py --config cfg.yaml` - the reference's training entry point on the H100-native hot path.
 
 `main(**yaml)` accepts the same keyword surface as the reference's `train.py:457-514`, so the v2 YAML configs load
-unchanged (keys this build does not act on - validation sampling, webui export, trackers - are accepted and ignored).
+unchanged (keys this build does not act on - trackers, text-encoder options it refuses - are accepted and ignored).
 What this file owns is the *step*: parameter selection (`handle_trainable_modules`, :316-337), LoRA injection through
 `LoraHandler` (:557-572), optimizer parameter groups (`create_optimizer_params`, :205-236), and per optimisation step:
 noise + timestep sampling (:751-757), the fused add_noise -> UNet fwd+bwd -> MSE step (`step.DataParallelStep`, two
@@ -13,7 +13,8 @@ classes (utils/dataset.py: OpenCV decode -> ONE resize + normalise kernel on the
 `cache_latents: True` writes / `cached_latent_dir` reads the reference's latent cache (`cached_{i}.pt`, train.py:266-314);
 `dataset_types: ['synthetic']` needs no files.  Prompts go through the frozen CLIP text encoder (text_encoder.py) with a
 per-prompt embedding cache; a batch that already carries `text_embeds` skips it.
-Checkpoints (8(f) row 4): LoRA in the cloneofsimo list format, the UNet in diffusers layout, and - when the pretrained folder
+Checkpoints (8(f) row 4): LoRA in the cloneofsimo list format or the stable_lora safetensors files (full weights and the webui
+file), the UNet in diffusers layout, and - when the pretrained folder
 is a full pipeline - the complete pipeline directory (`save_pipe`, train.py:395-449), plus a validation sample every
 `validation_steps` (sampling.py: DPM-Solver++ preview with the trained UNet in eval mode, train.py:908-958).
 """
@@ -432,13 +433,14 @@ def main(
 PIPELINE_PARTS = ("vae", "text_encoder", "tokenizer", "scheduler")
 
 
-def save_pipe(pretrained_model_path, unet, path):
+def save_pipe(pretrained_model_path, unet, path, unet_state_dict=None):
     """reference save_pipe (train.py:395-449): a complete TextToVideoSDPipeline directory - the trained UNet in diffusers
     layout plus the frozen parts and model_index.json of the pretrained pipeline, so `from_pretrained(path)` of a diffusers
-    pipeline (or train.main again) can load it.  A UNet-only pretrained folder yields a UNet-only checkpoint."""
+    pipeline (or train.main again) can load it.  A UNet-only pretrained folder yields a UNet-only checkpoint.
+    unet_state_dict: written instead of unet.state_dict() (stable LoRA: the merged weights)."""
     import shutil
     os.makedirs(path, exist_ok=True)
-    unet.save_pretrained(os.path.join(path, "unet"))
+    unet.save_pretrained(os.path.join(path, "unet"), state_dict=unet_state_dict)
     copied = []
     for part in PIPELINE_PARTS:
         src = os.path.join(pretrained_model_path, part)
@@ -459,26 +461,46 @@ def save_pipe(pretrained_model_path, unet, path):
 
 def save_checkpoint(unet, lora_manager, output_dir, step, use_unet_lora, save_pretrained_model, final=False, pretrained_model_path=None,
                     ema=None):
-    """LoRA in the cloneofsimo list format (`lora/<step>_unet.pt`) and, with save_pretrained_model, the pipeline directory.
-    ema (`use_ema`): the optimizer holding the EMA of the weights; the EMA weights are then written as well, as
-    `lora/<step>_unet_ema.pt` and (save_pretrained_model) `unet_ema/` in the diffusers UNet layout."""
+    """LoRA files and, with save_pretrained_model, the pipeline directory.
+      cloneofsimo: `lora/<step>_unet.pt` (list format).
+      stable_lora: `lora/full_weights/<step>_lora_text_to_video_unet.safetensors` (fp32) unless only_lora_for_webui, and with
+        save_lora_for_webui / only_lora_for_webui `lora/webui_<step>_lora_text_to_video.safetensors` (fp16, ModelScope keys).
+        `unet/` holds the delta merged into the base weights under the plain keys, so it loads into a plain UNet with
+        strict=True (the reference writes the lora_A / lora_B keys into unet/ as well, which a plain UNet load rejects).
+    ema (`use_ema`): the optimizer holding the EMA of the weights; the EMA weights are then written as well: the LoRA files
+    with an `_ema` suffix and (save_pretrained_model) `unet_ema/` in the diffusers UNet layout."""
     path = output_dir if final else os.path.join(output_dir, f"checkpoint-{step}")
     os.makedirs(path, exist_ok=True)
-    if use_unet_lora:   # the reference saves the LoRA files and (save_pretrained_model) the pipeline: train.py:908-958
-        from .utils.lora import save_lora_weight
-        os.makedirs(os.path.join(path, "lora"), exist_ok=True)
-        save_lora_weight(unet, os.path.join(path, "lora", f"{step}_unet.pt"), lora_manager.unet_replace_modules)
+    stable = use_unet_lora and lora_manager.is_stable_lora()
+    lora_dir = os.path.join(path, "lora")
+
+    def save_lora(suffix=""):
+        if not use_unet_lora:
+            return
+        os.makedirs(lora_dir, exist_ok=True)
+        if stable:
+            lora_manager.save_stable_lora(unet, lora_dir, step, suffix=suffix)
+        else:   # the reference saves the LoRA files and (save_pretrained_model) the pipeline: train.py:908-958
+            from .utils.lora import save_lora_weight
+            save_lora_weight(unet, os.path.join(lora_dir, f"{step}_unet{suffix}.pt"), lora_manager.unet_replace_modules)
+
+    def unet_sd():
+        if not stable:
+            return None
+        from .utils.stable_lora import merged_state_dict
+        return merged_state_dict(unet)
+
+    save_lora()
     if save_pretrained_model:
         if pretrained_model_path is not None:
-            save_pipe(pretrained_model_path, unet, path)
+            save_pipe(pretrained_model_path, unet, path, unet_state_dict=unet_sd())
         else:
-            unet.save_pretrained(os.path.join(path, "unet"))
+            unet.save_pretrained(os.path.join(path, "unet"), state_dict=unet_sd())
     if ema is not None:
         with ema.ema_weights():
-            if use_unet_lora:
-                save_lora_weight(unet, os.path.join(path, "lora", f"{step}_unet_ema.pt"), lora_manager.unet_replace_modules)
+            save_lora("_ema")
             if save_pretrained_model:
-                unet.save_pretrained(os.path.join(path, "unet_ema"))
+                unet.save_pretrained(os.path.join(path, "unet_ema"), state_dict=unet_sd())
 
 
 def load_config(path):

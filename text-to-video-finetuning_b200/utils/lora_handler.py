@@ -1,9 +1,19 @@
 """LoraHandler - the facade train.py uses to add / save LoRA adapters (reference utils/lora_handler.py:69-351).
 
 Same constructor keywords, `add_lora_to_model(...) -> (params, negation)`, `save_lora_weights(model, save_path, step)`,
-`deactivate_lora_train`, `LORA_VERSIONS`, and the cloneofsimo file layout (`<save_path>/lora/<step>_unet.pt`).
-Only the 'cloneofsimo' implementation is on the H100 hot path (BASELINE.json config 3); 'stable_lora' depends on the
-un-installed `loralib` package and raises a clear error instead of silently training something else.
+`deactivate_lora_train`, `LORA_VERSIONS`, and both file layouts: cloneofsimo (`<save_path>/lora/<step>_unet.pt`) and
+stable_lora (`<save_path>/lora/full_weights/<step>_lora_text_to_video_unet.safetensors`, plus the webui file
+`<save_path>/lora/webui_<step>_lora_text_to_video.safetensors`).  'stable_lora' (the reference's default) runs on
+utils/stable_lora.py; its UNet targets are Linear / Conv2d / Conv3d (the UNet has no nn.Embedding).
+
+Deviations from the reference, both so that a mistake fails instead of training something else:
+  * stable_lora `lora_path`: a file that is found but does not match the injected modules' keys and shapes raises
+    ValueError (the reference prints the error and trains fresh weights);
+  * injecting stable_lora into a model that already carries cloneofsimo wrappers raises NotImplementedError (the reference
+    would wrap the wrappers' own inner layers).
+`lora_bias` other than 'none' behaves as 'none' with a warning: the LoRA optimizer group only takes parameters whose name
+contains 'lora' (train.create_optimizer_params), so in the reference too a bias is only ever updated through
+`trainable_modules`, which sets its requires_grad itself.
 """
 import os
 import warnings
@@ -11,6 +21,7 @@ from types import SimpleNamespace
 
 import torch
 
+from . import stable_lora
 from .lora import (extract_lora_ups_down, inject_trainable_lora_extended, monkeypatch_or_replace_lora_extended,
                    save_lora_weight, train_patch_pipe)
 
@@ -32,11 +43,6 @@ LORA_FUNC_TYPES = [LoraFuncTypes.loader, LoraFuncTypes.injector]
 
 def filter_dict(_dict, keys=()):
     return {k: v for k, v in _dict.items() if k in keys}
-
-
-def _stable_lora_unavailable(*a, **k):
-    raise NotImplementedError("lora version 'stable_lora' needs the `loralib` package, which is not available in this "
-                              "build; use version 'cloneofsimo' (the configuration BASELINE.json benchmarks)")
 
 
 class LoraHandler(object):
@@ -67,7 +73,7 @@ class LoraHandler(object):
         if self.is_cloneofsimo_lora():
             return monkeypatch_or_replace_lora_extended if func_type == LoraFuncTypes.loader else inject_trainable_lora_extended
         if self.is_stable_lora():
-            return _stable_lora_unavailable
+            return stable_lora.load_lora if func_type == LoraFuncTypes.loader else stable_lora.add_lora_to
         raise ValueError(f"LoRA version {self.version!r} does not exist (choose from {LORA_VERSIONS})")
 
     def check_lora_ext(self, lora_file: str):
@@ -89,9 +95,22 @@ class LoraHandler(object):
             return dict(model=model, loras=self.get_lora_file_path(lora_path, model), target_replace_module=replace_modules, r=r)
         return dict(model=model, lora_path=lora_path)
 
+    def load_lora(self, model, lora_path=""):
+        """stable_lora: load the first LoRA file in `lora_path` whose name contains 'unet' (ValueError if it does not fit)."""
+        lora_file = self.get_lora_file_path(lora_path, model)
+        if lora_file is None:
+            if lora_path:
+                print(f"Could not load LoRAs for {model.__class__.__name__}. Injecting new ones instead...")
+            return
+        self.lora_loader(model, lora_file)
+        print(f"Successfully loaded LoRA from: {lora_file}")
+
     def do_lora_injection(self, model, replace_modules, bias="none", dropout=0, r=4, lora_loader_args=None):
         if self.is_stable_lora():
-            _stable_lora_unavailable()
+            search = [torch.nn.Linear, torch.nn.Conv2d, torch.nn.Conv3d, torch.nn.Embedding]
+            self.lora_injector(model, target_module=replace_modules, search_class=search, r=r, dropout=dropout,
+                               lora_bias=self.lora_bias)()
+            return None, None, False
         params, negation = self.lora_injector(**lora_loader_args)
         for up, down in extract_lora_ups_down(model, target_replace_module=replace_modules):
             if up is not None and down is not None:
@@ -103,13 +122,18 @@ class LoraHandler(object):
         params, negation = None, None
         args = self.get_lora_func_args(lora_path, use_lora, model, replace_modules, r, dropout, self.lora_bias)
         if use_lora:
-            params, negation, _ = self.do_lora_injection(model, replace_modules, bias=self.lora_bias, lora_loader_args=args,
-                                                         dropout=dropout, r=r)
+            params, negation, hybrid = self.do_lora_injection(model, replace_modules, bias=self.lora_bias, lora_loader_args=args,
+                                                              dropout=dropout, r=r)
+            if not hybrid:
+                self.load_lora(model, lora_path=lora_path)
         params = model if params is None else params
         return params, negation
 
     def deactivate_lora_train(self, models, deactivate=True):
-        """Only meaningful for stable_lora in the reference (:271-277); a no-op for cloneofsimo."""
+        """stable_lora: set the train/eval mode of the LoRA modules and of each model (reference set_mode_group, used
+        around previews); a no-op for cloneofsimo."""
+        if self.is_stable_lora():
+            stable_lora.set_mode_group(models, not deactivate)
 
     def save_cloneofsimo_lora(self, model, save_path, step):
         for name, cond, mods, sub in ((FILE_BASENAMES[0], self.use_unet_lora, self.unet_replace_modules, "unet"),
@@ -126,4 +150,11 @@ class LoraHandler(object):
                 warnings.warn("'save_for_webui' is only supported by the 'stable_lora' implementation")
             self.save_cloneofsimo_lora(model, save_path, step)
         if self.is_stable_lora():
-            _stable_lora_unavailable()
+            self.save_stable_lora(model.unet, save_path, step)
+
+    def save_stable_lora(self, unet, save_path, step, suffix=""):
+        """fp32 full weights and/or the fp16 webui file (see module docstring); returns the paths written."""
+        if self.lora_bias != "none":
+            warnings.warn(f"lora_bias={self.lora_bias!r} behaves as 'none' (only the lora_A / lora_B tensors are saved)")
+        return stable_lora.save_lora(unet, save_path, step, save_for_webui=self.save_for_webui, only_webui=self.only_for_webui,
+                                     suffix=suffix)
