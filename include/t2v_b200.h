@@ -237,6 +237,9 @@ int t2v_cast_f32_bf16(const float* src, void* dst, int64_t n, void* stream);
 int t2v_embed_tokens(const int64_t* ids, const float* tok_emb, const float* pos_emb, void* out, int64_t rows, int32_t L, int32_t C,
                      int32_t vocab, void* stream);
 int t2v_gelu_bf16(const void* x, void* y, int64_t n, int32_t quick, void* stream);
+/* Backward of t2v_gelu_bf16 for text-encoder LoRA training: dx = dy * gelu'(x), x the saved input, same `quick` switch;
+ * n a multiple of 8.                                                                                                     */
+int t2v_gelu_bwd_bf16(const void* x, const void* dy, void* dx, int64_t n, int32_t quick, void* stream);
 /* Data pipeline front end (reference utils/dataset.py:22-41 normalize_input after the video reader's resize): decoded RGB
  * frames uint8 [F][H0][W0][3] -> bilinear resize to h x w (half-pixel centres) -> x / 127.5 - 1 -> bf16 channels-last
  * [F][h][w][8] (channels 3..7 zero), the layout AutoencoderKL.encode consumes.                                          */

@@ -158,6 +158,29 @@ __global__ void gelu_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* 
         reinterpret_cast<uint4*>(y)[i] = pack8e(v);
     }
 }
+// dx = dy * gelu'(x): the backward of gelu_kernel, both forms (text-encoder LoRA training).  x is the saved fc1 output.
+//   quick_gelu: d/dx [x s(1.702 x)] = s + 1.702 x s (1 - s)
+__global__ void gelu_bwd_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ dy, __nv_bfloat16* __restrict__ dx,
+                                int64_t nvec, int quick) {
+    pdl_sync();
+    GRID_STRIDE(i, nvec) {
+        float v[8], d[8];
+        unpack8e(__ldg(reinterpret_cast<const uint4*>(x) + i), v);
+        unpack8e(__ldg(reinterpret_cast<const uint4*>(dy) + i), d);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            float g;
+            if (quick) {
+                const float s = sigm(1.702f * v[j]);
+                g = s + 1.702f * v[j] * s * (1.f - s);
+            } else {
+                g = gelu_erf_grad(v[j]);
+            }
+            d[j] *= g;
+        }
+        reinterpret_cast<uint4*>(dx)[i] = pack8e(d);
+    }
+}
 // out[b*L + l][:] = tok_emb[ids[b][l]][:] + pos_emb[l][:]   (fp32 tables -> bf16 activations; CLIPTextEmbeddings)
 __global__ void embed_tokens_kernel(const int64_t* __restrict__ ids, const float* __restrict__ tok, const float* __restrict__ pos,
                                     __nv_bfloat16* __restrict__ out, int64_t rows, int L, int C, int vocab) {
@@ -605,6 +628,11 @@ int t2v_gelu_bf16(const void* x, void* y, int64_t n, int32_t quick, void* stream
     if (n % 8) return fail(-2, "gelu: n must be a multiple of 8");
     launch_pdl(gelu_kernel, dim3(ew_grid(n / 8)), dim3(256), size_t(0), ST, BF(x), BFW(y), n / 8, quick);
     return launch_checked(int(cudaGetLastError()), "gelu_bf16");
+}
+int t2v_gelu_bwd_bf16(const void* x, const void* dy, void* dx, int64_t n, int32_t quick, void* stream) {
+    if (n % 8) return fail(-2, "gelu_bwd: n must be a multiple of 8");
+    launch_pdl(gelu_bwd_kernel, dim3(ew_grid(n / 8)), dim3(256), size_t(0), ST, BF(x), BF(dy), BFW(dx), n / 8, quick);
+    return launch_checked(int(cudaGetLastError()), "gelu_bwd_bf16");
 }
 int t2v_embed_tokens(const int64_t* ids, const float* tok_emb, const float* pos_emb, void* out, int64_t rows, int32_t L, int32_t C,
                      int32_t vocab, void* stream) {

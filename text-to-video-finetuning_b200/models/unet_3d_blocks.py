@@ -24,12 +24,16 @@ from ..layers import (Downsample2D, ResnetBlock2D, TemporalConvLayer, Transforme
 class StepContext:
     """Per-forward constants shared by all blocks."""
 
-    __slots__ = ("num_frames", "temb_act", "text")
+    __slots__ = ("num_frames", "temb_act", "text", "texts")
 
-    def __init__(self, num_frames, temb_act, text):
+    def __init__(self, num_frames, temb_act, text, texts=None):
         self.num_frames = num_frames  # F
         self.temb_act = temb_act      # SiLU(time embedding), bf16 [B, 4*C0]
         self.text = text              # bf16 [B*Lctx, ctx_dim]
+        self.texts = texts            # trainable text states: one ops.fork_f32 output per cross-attention, handed out in order
+
+    def take_text(self):
+        return self.texts.pop() if self.texts is not None else self.text
 
 
 def _maybe_ckpt(enabled, fn, *args):
@@ -79,7 +83,7 @@ class _Block3D(nn.Module):
 
     def _attn(self, m, h, sc):
         f = lambda t, c: m(t, c, num_frames=sc.num_frames).sample
-        return _maybe_ckpt(self.gradient_checkpointing, f, h, sc.text)
+        return _maybe_ckpt(self.gradient_checkpointing, f, h, sc.take_text())
 
     def _temp_attn(self, m, h, sc):
         if sc.num_frames <= 1:

@@ -14,7 +14,7 @@ import torch
 import torch.nn as nn
 
 from .. import ops, prims
-from ..layers import (TimestepEmbedding, Timesteps, TransformerTemporalModel, _channels_last_, clip_stats_rows, run_conv,
+from ..layers import (TimestepEmbedding, Timesteps, Transformer2DModel, TransformerTemporalModel, _channels_last_, clip_stats_rows, run_conv,
                       run_group_norm)
 from ..modeling_utils import ConfigMixin, ModelMixin, register_to_config
 from .unet_3d_blocks import (CrossAttnDownBlock3D, CrossAttnUpBlock3D, DownBlock3D, StepContext, UNetMidBlock3DCrossAttn,
@@ -135,7 +135,9 @@ class UNet3DConditionModel(ModelMixin, ConfigMixin):
         forward_upsample_size = any(s % (2 ** self.num_upsamplers) != 0 for s in (H, W))
 
         emb = self.time_embedding(self.time_proj(timesteps))
-        sc = StepContext(num_frames, ops.silu(emb), text)
+        # trainable text states (text-encoder LoRA): their gradient is summed over every cross-attention in fp32
+        texts = list(ops.fork_f32(text, self._n_cross_attention())) if text.requires_grad else None
+        sc = StepContext(num_frames, ops.silu(emb), text, texts)
 
         h = run_conv(self.conv_in, x, cin_pad=8 - cfg.in_channels, stats_rows=clip_stats_rows(num_frames, H * W))   # -> transformer_in (per clip)
         if num_frames > 1:
@@ -162,6 +164,9 @@ class UNet3DConditionModel(ModelMixin, ConfigMixin):
 
         h = run_group_norm(self.conv_norm_out, h, True, h.shape[0])
         return run_conv(self.conv_out, h, cout_pad=8 - cfg.out_channels)
+
+    def _n_cross_attention(self):
+        return sum(isinstance(m, Transformer2DModel) for m in self.modules())
 
     def forward(
         self,

@@ -146,6 +146,34 @@ class _Fork(Function):
         return acc, None
 
 
+class _ForkF32(Function):
+    """y_1 = ... = y_n = x with the n incoming gradients summed in fp32 (cast + add kernels) and rounded to bf16 once: the
+    text states feed the cross-attention K|V projection of every UNet transformer, a fan-in too wide for a bf16 sum."""
+
+    @staticmethod
+    def forward(ctx, x, n):
+        return tuple(x.view_as(x) for _ in range(n))
+
+    @staticmethod
+    def backward(ctx, *gs):
+        gs = [_cont(g) for g in gs if g is not None]
+        if not gs:
+            return None, None
+        acc = None
+        for g in gs:
+            g32 = torch.empty(g.shape, device=g.device, dtype=torch.float32)
+            prims.cast_bf16_f32(g, g32)
+            acc = g32 if acc is None else prims.add_f32(acc, g32)
+        return prims.cast_f32_bf16(acc), None
+
+
+def fork_f32(x, n):
+    """fork(x, n) whose backward accumulates the gradient in fp32 (bf16 x only)."""
+    if not x.requires_grad:
+        return (x,) * n
+    return _ForkF32.apply(x, n)
+
+
 def carry(dst, src):
     """GroupNorm input statistics travel with the activation as a Python attribute (`_t2v_stats`: list of fp32 tensors
     [frames, Ck, 2] covering consecutive channel ranges, filled by the epilogue of the GEMM that produced the activation).
@@ -450,6 +478,25 @@ def silu(x):
     return _Silu.apply(x)
 
 
+class _Gelu(Function):
+    """The text encoder's MLP activation: exact erf GELU or CLIP's quick_gelu."""
+
+    @staticmethod
+    def forward(ctx, x, quick):
+        ctx.save_for_backward(x)
+        ctx.quick = quick
+        return prims.gelu_bf16(x, quick=quick)
+
+    @staticmethod
+    def backward(ctx, dy):
+        (x,) = ctx.saved_tensors
+        return prims.gelu_bwd(x, _cont(dy), quick=ctx.quick), None
+
+
+def gelu(x, quick=False):
+    return _Gelu.apply(x, bool(quick))
+
+
 class _DropoutScaleAdd(Function):
     """base + scale * dropout_p(x) with a regenerated (not stored) mask."""
 
@@ -653,6 +700,45 @@ class _Attention(Function):
 
 def attention(q, k, v, heads):
     return _Attention.apply(q, k, v, heads)
+
+
+def causal_attention_fwd(q, k, v, heads):
+    """CLIP text self-attention, q/k/v [B, L, C] row-contiguous views: two batched GEMMs around the row softmax with the
+    causal mask (L = 77: launch-bound, no fused kernel).  Returns (o [B, L, C] bf16, P bf16 [B, heads, L, ld])."""
+    B, L, C = q.shape
+    D = C // heads
+    ld = _rup8(L)
+    s = torch.empty((B, heads, L, ld), device=q.device, dtype=torch.float32)
+    prims.bgemm(q, (1, q.stride(1), q.stride(0), D), k, (1, k.stride(1), k.stride(0), D), s, (ld, heads * L * ld, L * ld),
+                L, L, D, B, heads, D ** -0.5, 1)
+    p = prims.softmax_fwd(s, L, ld, causal_period=L)
+    del s
+    o = torch.empty((B, L, C), device=q.device, dtype=q.dtype)
+    prims.bgemm(p, (1, ld, heads * L * ld, L * ld), v, (0, v.stride(1), v.stride(0), D), o, (C, L * C, D), L, D, L, B, heads, 1.0, 0)
+    return o, p
+
+
+class _CausalAttention(Function):
+    """Backward: the unfused path of _attn_core_bwd on the stored probabilities; the masked ones are zero, so softmax_bwd
+    gives them a zero score gradient and the four GEMMs need no mask."""
+
+    @staticmethod
+    def forward(ctx, q, k, v, heads):
+        o, p = causal_attention_fwd(q, k, v, heads)
+        ctx.save_for_backward(q, k, v, p)
+        ctx.heads = heads
+        return o
+
+    @staticmethod
+    def backward(ctx, do):
+        q, k, v, p = ctx.saved_tensors
+        dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
+        _attn_core_bwd(q, k, v, p, _cont(do), dq, dk, dv, ctx.heads)
+        return dq, dk, dv, None
+
+
+def causal_attention(q, k, v, heads):
+    return _CausalAttention.apply(q, k, v, heads)
 
 
 class _AttentionFused(Function):

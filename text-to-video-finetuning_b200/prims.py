@@ -534,6 +534,15 @@ def gelu_bf16(x, quick=False):
     return y
 
 
+def gelu_bwd(x, dy, quick=False):
+    """dx = dy * gelu'(x) (bf16), the backward of gelu_bf16."""
+    _chk_bf16(x, dy)
+    assert x.shape == dy.shape
+    dx = torch.empty_like(x)
+    native.check(native.lib().t2v_gelu_bwd_bf16(_p(x), _p(dy), _p(dx), x.numel(), int(bool(quick)), _stream()))
+    return dx
+
+
 def frames_u8_to_nhwc8(frames, out_hw):
     """uint8 RGB frames [F, H0, W0, 3] -> bilinear resize + (x / 127.5 - 1) -> bf16 [F, h, w, 8] (VAE input layout)."""
     assert frames.dtype == torch.uint8 and frames.is_cuda and frames.is_contiguous() and frames.shape[-1] == 3, (frames.dtype, frames.shape)

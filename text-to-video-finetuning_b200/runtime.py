@@ -25,8 +25,10 @@ class ParamArena:
     only their storage moves.  `param.grad` becomes a view into the flat gradient buffer and matrix-like weights get a
     `_t2v_shadow` bf16 view in kernel layout ([Cout, KH, KW, Cin] / [out, 1, 1, in])."""
 
-    def __init__(self, module, device=None):
+    def __init__(self, module, device=None, extra=()):
+        # extra: parameters outside `module` to adopt as well (the text-encoder LoRA factors of a text-LoRA run)
         params = [p for p in module.parameters()]
+        params += [p for p in extra if all(p is not q for q in params)]
         if not params:
             raise ValueError("module has no parameters")
         device = device or params[0].device
@@ -147,7 +149,8 @@ class GradientBuckets:
     (down_blocks.i / mid_block / up_blocks.i) are one contiguous range.  The model marks the input of every block
     (ops.grad_mark); when the backward pass reaches a mark, that block's range is complete and its all-reduce is issued
     asynchronously (NCCL runs it on its own stream, also inside a captured CUDA graph) while the rest of the backward keeps
-    the SMs busy.  `finish()` reduces what is left of the trainable spans (stem, time embedding, all vectors) and joins.
+    the SMs busy.  `finish()` reduces what is left of the trainable spans (stem, time embedding, all vectors, and the text-encoder LoRA
+    factors, whose gradients are complete only once the text encoder's backward has run) and joins.
 
     compress (default on NCCL): gradients cross NVLink as bf16.  Each range is scaled by 1 / world and rounded into a flat
     bf16 twin of the gradient buffer (one pass, 6 B / parameter, overlapped like the collective itself), the SUM all-reduce

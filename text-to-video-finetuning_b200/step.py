@@ -121,17 +121,26 @@ class DataParallelStep:
         so neither a memset nor a cast pass remains in the step.  Without one (a torch optimizer, or fwd+bwd only) the
         buffer is zeroed at the start of each window and the shadow is re-cast from the masters every call.
 
-    `prediction_type` picks the loss target of every pass: the noise ('epsilon') or the velocity ('v_prediction')."""
+    `prediction_type` picks the loss target of every pass: the noise ('epsilon') or the velocity ('v_prediction').
+
+    `text_encoder` (a text_encoder.CLIPTextModel with cloneofsimo LoRA injected, `use_text_lora`): the call then takes the
+    prompt token ids (B, L) in place of the text states, and the step follows train.py:803-834: the encoder runs once, in
+    the step (and the graph); with passes=2 and F > 1, pass 0 is the full clip on the detached states and pass 1 only frame
+    1 of the clip on the trainable states - the one pass whose gradient reaches the text LoRA; with F = 1 one pass on the
+    trainable states.  The arena adopts the LoRA factors next to the UNet's parameters (never the frozen encoder weights),
+    so clipping, the optimizers and the EMA cover them."""
 
     def __init__(self, unet, alphas_cumprod, passes=1, use_graph=False, adopt=True, optimizer=None, accumulation=1,
-                 prediction_type="epsilon"):
+                 prediction_type="epsilon", text_encoder=None):
         if prediction_type not in PREDICTION_TYPES:
             raise ValueError(f"prediction_type {prediction_type!r} is not supported; expected one of {PREDICTION_TYPES}")
         self.unet = unet
         self.abar = alphas_cumprod
         self.prediction_type = prediction_type
         self.passes = passes
-        self.arena = ParamArena(unet) if adopt else None
+        self.text_encoder = text_encoder
+        text_params = [p for p in text_encoder.parameters() if p.requires_grad] if text_encoder is not None else ()
+        self.arena = ParamArena(unet, extra=text_params) if adopt else None
         self.use_graph = use_graph
         self.sync_gradients = True   # set False to run fwd+bwd only (profiling on a single rank)
         self.optimizer = optimizer
@@ -166,10 +175,19 @@ class DataParallelStep:
         total = None
         reduce_now = last and self.sync_gradients
         overlap = self.buckets is not None and reduce_now
-        for i in range(self.passes):
-            loss = finetune_loss(self.unet, latents, noise, timesteps, text, self.abar, prediction_type=self.prediction_type)
+        if self.text_encoder is None:
+            runs = [(latents, noise, text)] * self.passes
+        else:
+            B, L = text.shape                              # text = prompt token ids
+            states = self.text_encoder.encode(text).view(B, L, -1)
+            if self.passes > 1 and latents.shape[2] > 1:
+                runs = [(latents, noise, states.detach()), (latents[:, :, 1:2], noise[:, :, 1:2], states)]
+            else:
+                runs = [(latents, noise, states)]
+        for i, (lat, nz, st) in enumerate(runs):
+            loss = finetune_loss(self.unet, lat, nz, timesteps, st, self.abar, prediction_type=self.prediction_type)
             if overlap:
-                self.buckets.armed = i == self.passes - 1   # gradients are final only in the last pass
+                self.buckets.armed = i == len(runs) - 1   # gradients are final only in the last pass
             loss.backward(self._gscale if self.accumulation > 1 else None)
             total = loss.detach() if total is None else total + loss.detach()
         comm = None
@@ -186,6 +204,7 @@ class DataParallelStep:
         return total
 
     def __call__(self, latents, noise, timesteps, encoder_hidden_states):
+        """encoder_hidden_states: the text states (B, L, D), or with a text encoder attached its token ids (B, L)."""
         if self.arena is not None:
             self.arena.check_layout()
             self.arena.reattach_grads()

@@ -1,14 +1,19 @@
-"""Frozen CLIP text encoder on the H100-native kernels - SURVEY 8(f) row 2 (`text_encoder(token_ids)[0]`, train.py:784-790).
+"""CLIP text encoder on the H100-native kernels - SURVEY 8(f) row 2 (`text_encoder(token_ids)[0]`, train.py:784-790).
 
 Drop-in for the `transformers.CLIPTextModel` the reference loads with `CLIPTextModel.from_pretrained(path,
-subfolder="text_encoder")` (train.py:120): same parameter names (a Hugging Face checkpoint loads unchanged), same call
-`model(input_ids)[0]` -> last_hidden_state (B, L, hidden).  Forward only: the text encoder is frozen on the finetune path
-(train_text_encoder / use_text_lora are outside this build and rejected by train.main).
+subfolder="text_encoder")` (train.py:120): same parameter names and module class names (a Hugging Face checkpoint loads
+unchanged, and LoRA injection finds `CLIPEncoderLayer` / `CLIPAttention` / `CLIPMLP` by class name as it does on the
+transformers model), same call `model(input_ids)[0]` -> last_hidden_state (B, L, hidden).
 
-Per layer: LayerNorm -> fused Q|K|V GEMM (weights concatenated once: the encoder is frozen) -> causal attention (two batched
-wgmma GEMMs around the row-softmax kernel with the causal mask; L = 77 makes this launch-bound, not worth a fused kernel)
--> output projection with the residual in the GEMM epilogue -> LayerNorm -> fc1 -> GELU -> fc2 (+ residual epilogue).
-Embedding lookup (token + position) is one kernel; final LayerNorm as in CLIPTextTransformer."""
+Frozen encoder (no LoRA injected): a no-grad forward.  Per layer: LayerNorm -> fused Q|K|V GEMM (weights concatenated once)
+-> causal attention (two batched wgmma GEMMs around the row-softmax kernel with the causal mask; L = 77 makes this
+launch-bound, not worth a fused kernel) -> output projection with the residual in the GEMM epilogue -> LayerNorm -> fc1 ->
+GELU -> fc2 (+ residual epilogue).  Embedding lookup (token + position) is one kernel; final LayerNorm as in
+CLIPTextTransformer.
+
+Encoder with cloneofsimo LoRA wrappers (`use_text_lora`, train.py:571-572): `encode` runs the same layers as autograd ops
+(ops.py), each projection through its wrapper (utils/lora.lora_linear_forward), so the LoRA factors get gradients and the
+eval forward applies them.  The frozen base weights are cast to bf16 once (`_t2v_shadow`); no embedding gradient is formed."""
 import json
 import os
 from types import SimpleNamespace
@@ -19,45 +24,46 @@ import torch.nn as nn
 from . import ops, prims
 
 
-class _Attn(nn.Module):
+class CLIPAttention(nn.Module):
     def __init__(self, C):
         super().__init__()
-        self.q_proj, self.k_proj, self.v_proj, self.out_proj = (nn.Linear(C, C) for _ in range(4))
+        # transformers' registration order: LoRA files list the wrapped projections in module order
+        self.k_proj, self.v_proj, self.q_proj, self.out_proj = (nn.Linear(C, C) for _ in range(4))
 
 
-class _Mlp(nn.Module):
+class CLIPMLP(nn.Module):
     def __init__(self, C, I):
         super().__init__()
         self.fc1, self.fc2 = nn.Linear(C, I), nn.Linear(I, C)
 
 
-class _Layer(nn.Module):
+class CLIPEncoderLayer(nn.Module):
     def __init__(self, C, I, eps):
         super().__init__()
-        self.self_attn = _Attn(C)
+        self.self_attn = CLIPAttention(C)
         self.layer_norm1 = nn.LayerNorm(C, eps=eps)
-        self.mlp = _Mlp(C, I)
+        self.mlp = CLIPMLP(C, I)
         self.layer_norm2 = nn.LayerNorm(C, eps=eps)
 
 
-class _Embeddings(nn.Module):
+class CLIPTextEmbeddings(nn.Module):
     def __init__(self, vocab, positions, C):
         super().__init__()
         self.token_embedding = nn.Embedding(vocab, C)
         self.position_embedding = nn.Embedding(positions, C)
 
 
-class _Encoder(nn.Module):
+class CLIPEncoder(nn.Module):
     def __init__(self, n, C, I, eps):
         super().__init__()
-        self.layers = nn.ModuleList([_Layer(C, I, eps) for _ in range(n)])
+        self.layers = nn.ModuleList([CLIPEncoderLayer(C, I, eps) for _ in range(n)])
 
 
-class _TextTransformer(nn.Module):
+class CLIPTextTransformer(nn.Module):
     def __init__(self, cfg):
         super().__init__()
-        self.embeddings = _Embeddings(cfg.vocab_size, cfg.max_position_embeddings, cfg.hidden_size)
-        self.encoder = _Encoder(cfg.num_hidden_layers, cfg.hidden_size, cfg.intermediate_size, cfg.layer_norm_eps)
+        self.embeddings = CLIPTextEmbeddings(cfg.vocab_size, cfg.max_position_embeddings, cfg.hidden_size)
+        self.encoder = CLIPEncoder(cfg.num_hidden_layers, cfg.hidden_size, cfg.intermediate_size, cfg.layer_norm_eps)
         self.final_layer_norm = nn.LayerNorm(cfg.hidden_size, eps=cfg.layer_norm_eps)
 
 
@@ -76,7 +82,7 @@ class CLIPTextModel(nn.Module):
             raise NotImplementedError(f"hidden_act {self.config.hidden_act!r}")
         if self.config.hidden_size % self.config.num_attention_heads or self.config.hidden_size % 8:
             raise ValueError("hidden_size must be a multiple of the head count and of 8")
-        self.text_model = _TextTransformer(self.config)
+        self.text_model = CLIPTextTransformer(self.config)
         self.requires_grad_(False)
         self._packed = None
 
@@ -98,6 +104,8 @@ class CLIPTextModel(nn.Module):
 
     def load_state_dict(self, state_dict, strict=True):
         self._packed = None
+        for p in self.parameters():
+            p.__dict__.pop("_t2v_shadow", None)
         return super().load_state_dict(state_dict, strict=strict)
 
     @property
@@ -121,10 +129,76 @@ class CLIPTextModel(nn.Module):
         self._packed = dict(device=device, layers=layers)
         return self._packed
 
-    @torch.no_grad()
+    def lora_injected(self):
+        from .utils.lora import _WRAPPERS
+        return any(isinstance(m, _WRAPPERS) for m in self.modules())
+
     def forward(self, input_ids, attention_mask=None, **unused):
         """input_ids (B, L) int64 -> (last_hidden_state (B, L, hidden) fp32,).  The causal mask is always applied and, like
-        the reference's call (train.py:786), no padding mask is."""
+        the reference's call (train.py:786), no padding mask is.  With LoRA injected this is `encode` (differentiable)."""
+        if self.lora_injected():
+            B, L = input_ids.shape
+            return (self.encode(input_ids).float().view(B, L, -1),)
+        return self._forward_frozen(input_ids)
+
+    def _frozen_shadows(self):
+        """bf16 kernel-layout copies of the frozen projection weights, made once and read by ops.weight_bf16."""
+        for m in self.text_model.encoder.modules():
+            w = getattr(m, "weight", None)
+            if type(m) is not nn.Linear or w.requires_grad:
+                continue
+            sh = getattr(w, "_t2v_shadow", None)
+            if sh is None or sh.device != w.device:
+                w._t2v_shadow = prims.cast_f32_bf16(w.detach().float().contiguous()).view(w.shape[0], 1, 1, w.shape[1])
+
+    def encode(self, input_ids):
+        """Autograd forward of an encoder with LoRA wrappers: input_ids (B, L) -> bf16 token matrix [B*L, hidden], the
+        final-LayerNorm output.  Gradients reach the LoRA factors only (base weights, norms and embeddings are frozen)."""
+        from .layers import run_linear
+        cfg = self.config
+        ids = input_ids.to(torch.int64).contiguous()
+        B, L = ids.shape
+        C, H = cfg.hidden_size, cfg.num_attention_heads
+        quick = cfg.hidden_act == "quick_gelu"
+        emb = self.text_model.embeddings
+        self._frozen_shadows()
+        x = prims.embed_tokens(ids, emb.token_embedding.weight.detach().float().contiguous(),
+                               emb.position_embedding.weight.detach().float().contiguous())          # [B*L, C] bf16
+        for lyr in self.text_model.encoder.layers:
+            a, ln1, ln2 = lyr.self_attn, lyr.layer_norm1, lyr.layer_norm2
+            res, h = ops.fork(x)
+            n1, n2, n3 = ops.fork(ops.layer_norm(h, ln1.weight, ln1.bias, ln1.eps), 3)
+            q, k, v = (run_linear(m, t).view(B, L, C) for m, t in ((a.q_proj, n1), (a.k_proj, n2), (a.v_proj, n3)))
+            x = run_linear(a.out_proj, ops.causal_attention(q, k, v, H).view(B * L, C), residual=res)
+            res, h = ops.fork(x)
+            h = ops.gelu(run_linear(lyr.mlp.fc1, ops.layer_norm(h, ln2.weight, ln2.bias, ln2.eps)), quick)
+            x = run_linear(lyr.mlp.fc2, h, residual=res)
+        fl = self.text_model.final_layer_norm
+        return ops.layer_norm(x, fl.weight, fl.bias, fl.eps)
+
+    def plain_state_dict(self):
+        """fp32 CPU state dict under the plain Hugging Face keys, every cloneofsimo LoRA collapsed into its base weight
+        (W + scale * up @ down): it loads with strict=True into transformers.CLIPTextModel and into this class."""
+        from .utils.lora import _WRAPPERS
+        wrappers = {n: m for n, m in self.named_modules() if isinstance(m, _WRAPPERS)}
+        sd = {}
+        for k, v in self.state_dict().items():
+            head, _, leaf = k.rpartition(".")
+            parent, _, child = head.rpartition(".")
+            if parent in wrappers:
+                if child == "linear":
+                    sd[f"{parent}.{leaf}"] = v
+                continue
+            sd[k] = v
+        for n, m in wrappers.items():
+            up, down = m.lora_up.weight.detach().float(), m.lora_down.weight.detach().float()
+            if not isinstance(m.selector, nn.Identity):
+                down = m.selector.weight.detach().float() @ down
+            sd[f"{n}.weight"] = m.linear.weight.detach().float() + m.scale * (up @ down)
+        return {k: v.detach().float().cpu().contiguous() for k, v in sd.items()}
+
+    @torch.no_grad()
+    def _forward_frozen(self, input_ids):
         cfg = self.config
         ids = input_ids.to(torch.int64).contiguous()
         B, L = ids.shape

@@ -12,7 +12,8 @@ Data (SURVEY 8(f) rows 2-3): `dataset_types` in ('json', 'single_video', 'image'
 classes (utils/dataset.py: OpenCV decode -> ONE resize + normalise kernel on the GPU -> batched AutoencoderKL.encode);
 `cache_latents: True` writes / `cached_latent_dir` reads the reference's latent cache (`cached_{i}.pt`, train.py:266-314);
 `dataset_types: ['synthetic']` needs no files.  Prompts go through the frozen CLIP text encoder (text_encoder.py) with a
-per-prompt embedding cache; a batch that already carries `text_embeds` skips it.
+per-prompt embedding cache; a batch that already carries `text_embeds` skips it.  `use_text_lora` (cloneofsimo only) injects
+LoRA into the text encoder (train.py:571-572) and runs it inside the step on every batch's `prompt_ids` (step.py).
 Checkpoints (8(f) row 4): LoRA in the cloneofsimo list format or the stable_lora safetensors files (full weights and the webui
 file), the UNet in diffusers layout, and - when the pretrained folder
 is a full pipeline - the complete pipeline directory (`save_pipe`, train.py:395-449), plus a validation sample every
@@ -247,8 +248,12 @@ def main(
     if world > 1 and not dist.is_initialized():
         os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
         dist.init_process_group("nccl", device_id=dev)
-    if train_text_encoder or use_text_lora:
-        raise NotImplementedError("text-encoder training is outside the H100 hot path of this build (SURVEY 8(f) row 2)")
+    if train_text_encoder:
+        raise NotImplementedError("train_text_encoder (full text-encoder training) is not implemented; use_text_lora with "
+                                  "lora_version 'cloneofsimo' trains a LoRA of the text encoder")
+    if use_text_lora and lora_version == "stable_lora":
+        raise NotImplementedError("use_text_lora is implemented for lora_version 'cloneofsimo' only")
+    # text_encoder_gradient_checkpointing is accepted and has no effect: the text activations are 77 tokens per prompt
     fused_adamw = bool(kwargs.get("fused_adamw", True))   # optim.FusedAdamW on the flat arena (SURVEY 8(f) row 1); False: torch AdamW
     if use_8bit_adam and not fused_adamw:
         raise ValueError("use_8bit_adam runs optim.AdamW8bit on the flat arena; it cannot be combined with fused_adamw=False")
@@ -278,29 +283,43 @@ def main(
     if scale_lr:
         learning_rate = learning_rate * gradient_accumulation_steps * train_batch_size * world
 
-    lora_manager = LoraHandler(version=lora_version, use_unet_lora=use_unet_lora, use_text_lora=False,
+    lora_manager = LoraHandler(version=lora_version, use_unet_lora=use_unet_lora, use_text_lora=use_text_lora,
                                save_for_webui=save_lora_for_webui, only_for_webui=only_lora_for_webui,
                                unet_replace_modules=list(unet_lora_modules),
                                text_encoder_replace_modules=list(text_encoder_lora_modules), lora_bias=lora_bias)
     unet_lora_params, unet_negation = lora_manager.add_lora_to_model(use_unet_lora, unet, lora_manager.unet_replace_modules,
                                                                      lora_unet_dropout, lora_path, r=lora_rank)
+    text_encoder = text_lora_params = None
+    if use_text_lora:   # the text encoder and its LoRA must exist before the parameter arena is built
+        from .text_encoder import CLIPTextModel
+        text_encoder = _load_optional(CLIPTextModel, pretrained_model_path, "text_encoder")
+        if text_encoder is None:
+            raise FileNotFoundError(f"use_text_lora needs the text encoder of the pipeline: {pretrained_model_path}/text_encoder is missing")
+        text_lora_params, _ = lora_manager.add_lora_to_model(True, text_encoder, lora_manager.text_encoder_replace_modules,
+                                                             lora_text_dropout, lora_path, r=lora_rank)
+        text_encoder = text_encoder.to(dev).train()
     unet = unet.to(dev)
     unet.train()
     if kwargs.get("eval_train", False):  # train.py:779-781
         unet.eval()
+        if text_encoder is not None:
+            text_encoder.eval()
     handle_trainable_modules(unet, trainable_modules, is_enabled=True, negation=unet_negation)
     unet._set_gradient_checkpointing(gradient_checkpointing)
 
     extra_unet_params = extra_unet_params or {}
+    # train.py:581-595: UNet, text encoder (train_text_encoder only, refused above), text LoRA, UNet LoRA; the text LoRA group
+    # takes extra_unet_params, as in the reference (SURVEY H4)
     groups = create_optimizer_params([
         param_optim(unet, trainable_modules is not None, extra_params=extra_unet_params, negation=unet_negation),
+        param_optim(text_lora_params, use_text_lora, is_lora=True, extra_params={**{"lr": learning_rate}, **extra_unet_params}),
         param_optim(unet_lora_params, use_unet_lora, is_lora=True, extra_params={**{"lr": learning_rate}, **extra_unet_params}),
     ], learning_rate)
 
     abar = abar.to(dev)
     use_graph = bool(kwargs.get("use_cuda_graph", dev.type == "cuda"))   # replay the whole step as one CUDA graph (static shapes)
     stepper = DataParallelStep(unet, abar, passes=2, use_graph=use_graph, accumulation=gradient_accumulation_steps,
-                               prediction_type=prediction_type)
+                               prediction_type=prediction_type, text_encoder=text_encoder)
     # parameters now live in the flat arena.  Every rank must start from rank 0's weights (DDP does this at wrap time).
     if world > 1:
         dist.broadcast(stepper.arena.master, src=0)
@@ -322,20 +341,22 @@ def main(
 
     kinds = [dataset_types] if isinstance(dataset_types, str) else list(dataset_types)
     # frozen side models, loaded only when the pretrained folder has them (a UNet-only folder trains from latents + embeddings)
-    vae = text_encoder = tokenizer = None
+    vae = tokenizer = None
     if dev.type == "cuda" or kwargs.get("load_side_models"):
         from .text_encoder import CLIPTextModel
         from .vae import AutoencoderKL
         vae = _load_optional(AutoencoderKL, pretrained_model_path, "vae")
-        text_encoder = _load_optional(CLIPTextModel, pretrained_model_path, "text_encoder")
         if vae is not None:
             vae = vae.to(dev).eval()
-        if text_encoder is not None:
-            text_encoder = text_encoder.to(dev).eval()
+        if text_encoder is None:
+            text_encoder = _load_optional(CLIPTextModel, pretrained_model_path, "text_encoder")
+            if text_encoder is not None:
+                text_encoder = text_encoder.to(dev).eval()
         if os.path.isdir(os.path.join(pretrained_model_path, "tokenizer")):
             from transformers import CLIPTokenizer
             tokenizer = CLIPTokenizer.from_pretrained(pretrained_model_path, subfolder="tokenizer")
-    embed_text = TextEmbedder(text_encoder, dev) if text_encoder is not None else None
+    # a text encoder that trains is run by the step on every batch: no embedding cache
+    embed_text = TextEmbedder(text_encoder, dev) if text_encoder is not None and not use_text_lora else None
     if cached_latent_dir:
         dataset = CachedLatents(cached_latent_dir)
     elif "synthetic" in kinds:
@@ -380,7 +401,12 @@ def main(
                 latents = frames_to_latents(batch, vae, dev)        # raw clip -> resize/normalise kernel -> batched VAE encode
             else:
                 latents = batch["pixel_values"].to(dev, torch.float32)
-            if "text_embeds" in batch:
+            if use_text_lora:   # the step encodes the token ids itself
+                if "prompt_ids" not in batch:
+                    raise ValueError("use_text_lora trains the text encoder, so every batch needs 'prompt_ids'; this one has "
+                                     f"{sorted(batch)} (the synthetic dataset and a latent cache of text_embeds only have none)")
+                text = batch["prompt_ids"].reshape(latents.shape[0], -1).to(dev, torch.int64)
+            elif "text_embeds" in batch:
                 text = batch["text_embeds"].to(dev, torch.float32)
             elif embed_text is not None and "prompt_ids" in batch:
                 text = embed_text(batch["prompt_ids"])                # frozen CLIP text encoder, cached per prompt
@@ -412,11 +438,13 @@ def main(
                 print(f"step {global_step}/{max_train_steps} loss {loss.item():.5f} ({(time.time() - t0) / global_step:.3f} s/step)")
             if rank == 0 and global_step % checkpointing_steps == 0:
                 save_checkpoint(unet, lora_manager, output_dir, global_step, use_unet_lora, save_pretrained_model,
-                                pretrained_model_path=pretrained_model_path, ema=optimizer if use_ema else None)
+                                pretrained_model_path=pretrained_model_path, ema=optimizer if use_ema else None,
+                                text_encoder=text_encoder if use_text_lora else None)
             if rank == 0 and validation_data and validation_steps and global_step % validation_steps == 0 and vae is not None \
                     and text_encoder is not None and tokenizer is not None and getattr(vae, "decoder", None) is not None:
                 from .sampling import validation_sample
-                with optimizer.ema_weights() if use_ema else contextlib.nullcontext():   # preview what a user would export
+                with optimizer.ema_weights() if use_ema else contextlib.nullcontext(), \
+                        _text_preview(text_encoder) if use_text_lora else contextlib.nullcontext():   # preview what a user would export
                     validation_sample(unet, vae, text_encoder, tokenizer, validation_data, os.path.join(output_dir, "samples"), global_step,
                                       batch.get("text_prompt", [""])[0] if isinstance(batch.get("text_prompt"), (list, tuple)) else "",
                                       dev, alphas_cumprod=abar, prediction_type=prediction_type)
@@ -426,8 +454,21 @@ def main(
         dist.barrier()
     if rank == 0:
         save_checkpoint(unet, lora_manager, output_dir, global_step, use_unet_lora, save_pretrained_model, final=True,
-                        pretrained_model_path=pretrained_model_path, ema=optimizer if use_ema else None)
+                        pretrained_model_path=pretrained_model_path, ema=optimizer if use_ema else None,
+                        text_encoder=text_encoder if use_text_lora else None)
     return {"steps": global_step, "step_times": step_times, "stepper": stepper, "optimizer": optimizer}
+
+
+@contextlib.contextmanager
+def _text_preview(text_encoder):
+    """The validation preview encodes through the LoRA text encoder in eval mode (LoRA dropout off) and without a tape."""
+    was = text_encoder.training
+    text_encoder.eval()
+    try:
+        with torch.no_grad():
+            yield
+    finally:
+        text_encoder.train(was)
 
 
 PIPELINE_PARTS = ("vae", "text_encoder", "tokenizer", "scheduler")
@@ -460,7 +501,7 @@ def save_pipe(pretrained_model_path, unet, path, unet_state_dict=None):
 
 
 def save_checkpoint(unet, lora_manager, output_dir, step, use_unet_lora, save_pretrained_model, final=False, pretrained_model_path=None,
-                    ema=None):
+                    ema=None, text_encoder=None):
     """LoRA files and, with save_pretrained_model, the pipeline directory.
       cloneofsimo: `lora/<step>_unet.pt` (list format).
       stable_lora: `lora/full_weights/<step>_lora_text_to_video_unet.safetensors` (fp32) unless only_lora_for_webui, and with
@@ -468,13 +509,20 @@ def save_checkpoint(unet, lora_manager, output_dir, step, use_unet_lora, save_pr
         `unet/` holds the delta merged into the base weights under the plain keys, so it loads into a plain UNet with
         strict=True (the reference writes the lora_A / lora_B keys into unet/ as well, which a plain UNet load rejects).
     ema (`use_ema`): the optimizer holding the EMA of the weights; the EMA weights are then written as well: the LoRA files
-    with an `_ema` suffix and (save_pretrained_model) `unet_ema/` in the diffusers UNet layout."""
+    with an `_ema` suffix and (save_pretrained_model) `unet_ema/` in the diffusers UNet layout.
+    text_encoder (`use_text_lora`): `lora/<step>_text_encoder.pt` (and `_ema`) in the same list format, and with
+    save_pretrained_model `text_encoder/model.safetensors` holding the LoRA collapsed into the plain Hugging Face keys (the
+    reference writes the wrapper keys, which transformers.CLIPTextModel does not load as the trained encoder)."""
     path = output_dir if final else os.path.join(output_dir, f"checkpoint-{step}")
     os.makedirs(path, exist_ok=True)
     stable = use_unet_lora and lora_manager.is_stable_lora()
     lora_dir = os.path.join(path, "lora")
 
     def save_lora(suffix=""):
+        if text_encoder is not None:
+            from .utils.lora import save_lora_weight
+            os.makedirs(lora_dir, exist_ok=True)
+            save_lora_weight(text_encoder, os.path.join(lora_dir, f"{step}_text_encoder{suffix}.pt"), lora_manager.text_encoder_replace_modules)
         if not use_unet_lora:
             return
         os.makedirs(lora_dir, exist_ok=True)
@@ -496,6 +544,12 @@ def save_checkpoint(unet, lora_manager, output_dir, step, use_unet_lora, save_pr
             save_pipe(pretrained_model_path, unet, path, unet_state_dict=unet_sd())
         else:
             unet.save_pretrained(os.path.join(path, "unet"), state_dict=unet_sd())
+        if text_encoder is not None and os.path.isdir(os.path.join(path, "text_encoder")):
+            from safetensors.torch import save_file
+            te_dir = os.path.join(path, "text_encoder")
+            if os.path.isfile(os.path.join(te_dir, "pytorch_model.bin")):   # the pretrained weights copied by save_pipe
+                os.remove(os.path.join(te_dir, "pytorch_model.bin"))
+            save_file(text_encoder.plain_state_dict(), os.path.join(te_dir, "model.safetensors"), metadata={"format": "pt"})
     if ema is not None:
         with ema.ema_weights():
             save_lora("_ema")
