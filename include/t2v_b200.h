@@ -244,6 +244,13 @@ int t2v_gelu_bwd_bf16(const void* x, const void* dy, void* dx, int64_t n, int32_
  * frames uint8 [F][H0][W0][3] -> bilinear resize to h x w (half-pixel centres) -> x / 127.5 - 1 -> bf16 channels-last
  * [F][h][w][8] (channels 3..7 zero), the layout AutoencoderKL.encode consumes.                                          */
 int t2v_frames_u8_to_nhwc8(const uint8_t* src, void* dst, int32_t F, int32_t H0, int32_t W0, int32_t h, int32_t w, void* stream);
+/* The same for a ragged batch (train_batch_size > 1 on clips of different native sizes), in one launch: `src` packs every
+ * clip's uint8 [F_k][H0_k][W0_k][3] frames back to back; `table` (device, int64 [n_clips][4]) holds per clip its byte offset
+ * in `src`, F_k, H0_k and W0_k; total_frames = sum of F_k.  dst = bf16 [total_frames][h][w][8], clip after clip, each
+ * clip's slice bitwise equal to t2v_frames_u8_to_nhwc8 on that clip alone.  1 <= n_clips <= 256; the table's rows are
+ * trusted (prims.frames_u8_to_nhwc8_ragged checks them against the buffer size before the launch).                     */
+int t2v_frames_u8_to_nhwc8_ragged(const uint8_t* src, const int64_t* table, int32_t n_clips, int64_t total_frames, void* dst, int32_t h,
+                                  int32_t w, void* stream);
 /* Gradient compression around the data-parallel all-reduce (the reference reduces through accelerate/DDP, train.py:661,861):
  * dst (bf16) = alpha * src (fp32), alpha = 1 / world so that a SUM all-reduce averages; and the widening inverse.          */
 int t2v_scale_cast_f32_bf16(const float* src, void* dst, int64_t n, float alpha, void* stream);

@@ -303,6 +303,24 @@ __global__ void cast_f32_bf16_kernel(const float* __restrict__ src, __nv_bfloat1
 // Data pipeline (SURVEY 8(f) row 3; reference utils/dataset.py:22-41 normalize_input + the decoder's resize): decoded RGB frames
 // uint8 [F][H0][W0][3] -> bilinear resize (half-pixel centres, as F.interpolate(align_corners=False)) -> x / 127.5 - 1 ->
 // bf16 channels-last [F][h][w][8] (channels 3..7 zero): exactly the tensor AutoencoderKL.encode consumes, in one pass.
+// One output pixel (x, y) of the frame at `base` [H0][W0][3]; sy = H0 / h, sx = W0 / w.  Both resize kernels below call this,
+// so a clip resized inside a ragged batch is bitwise equal to the same clip resized alone.
+__device__ __forceinline__ uint4 bilinear_px8(const uint8_t* __restrict__ base, int H0, int W0, float sy, float sx, int x, int y) {
+    const float fy = fmaxf((y + 0.5f) * sy - 0.5f, 0.f), fx = fmaxf((x + 0.5f) * sx - 0.5f, 0.f);
+    const int y0 = min(int(fy), H0 - 1), x0 = min(int(fx), W0 - 1);
+    const int y1 = min(y0 + 1, H0 - 1), x1 = min(x0 + 1, W0 - 1);
+    const float wy = fy - float(y0), wx = fx - float(x0);
+    float v[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        const float p00 = base[(int64_t(y0) * W0 + x0) * 3 + c], p01 = base[(int64_t(y0) * W0 + x1) * 3 + c];
+        const float p10 = base[(int64_t(y1) * W0 + x0) * 3 + c], p11 = base[(int64_t(y1) * W0 + x1) * 3 + c];
+        const float top = p00 + (p01 - p00) * wx, bot = p10 + (p11 - p10) * wx;
+        v[c] = (top + (bot - top) * wy) * (1.0f / 127.5f) - 1.0f;
+    }
+    return pack8e(v);
+}
+
 __global__ void frames_u8_to_nhwc8_kernel(const uint8_t* __restrict__ src, __nv_bfloat16* __restrict__ dst, int F, int H0, int W0, int h, int w) {
     pdl_sync();
     const int64_t total = int64_t(F) * h * w;
@@ -310,20 +328,52 @@ __global__ void frames_u8_to_nhwc8_kernel(const uint8_t* __restrict__ src, __nv_
     GRID_STRIDE(i, total) {
         const int x = int(i % w), y = int((i / w) % h);
         const int f = int(i / (int64_t(w) * h));
-        const float fy = fmaxf((y + 0.5f) * sy - 0.5f, 0.f), fx = fmaxf((x + 0.5f) * sx - 0.5f, 0.f);
-        const int y0 = min(int(fy), H0 - 1), x0 = min(int(fx), W0 - 1);
-        const int y1 = min(y0 + 1, H0 - 1), x1 = min(x0 + 1, W0 - 1);
-        const float wy = fy - float(y0), wx = fx - float(x0);
-        const uint8_t* base = src + int64_t(f) * H0 * W0 * 3;
-        float v[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-            const float p00 = base[(int64_t(y0) * W0 + x0) * 3 + c], p01 = base[(int64_t(y0) * W0 + x1) * 3 + c];
-            const float p10 = base[(int64_t(y1) * W0 + x0) * 3 + c], p11 = base[(int64_t(y1) * W0 + x1) * 3 + c];
-            const float top = p00 + (p01 - p00) * wx, bot = p10 + (p11 - p10) * wx;
-            v[c] = (top + (bot - top) * wy) * (1.0f / 127.5f) - 1.0f;
+        reinterpret_cast<uint4*>(dst)[i] = bilinear_px8(src + int64_t(f) * H0 * W0 * 3, H0, W0, sy, sx, x, y);
+    }
+}
+
+// The same resize for a ragged batch of clips in ONE launch: clip k has F_k frames of its own native size H0_k x W0_k, stored
+// at byte `offset_k` of one packed buffer; table = int64 [n_clips][4] (offset, F, H0, W0).  Output bf16 [sum F_k][h][w][8],
+// clip after clip.  Every block stages the table in shared memory with the clips' first output frames (prefix sum of F) and
+// scales, then walks output pixels grid-stride; a pixel finds its clip by binary search over the first frames.  Idx: the pixel
+// index type - 32-bit whenever the output has < 2^31 pixels (every training batch), which turns the index divisions into
+// 32-bit ones; 64-bit otherwise.
+constexpr int kRaggedMaxClips = 256;
+template <typename Idx>
+__global__ void __launch_bounds__(256) frames_u8_to_nhwc8_ragged_kernel(const uint8_t* __restrict__ src, const int64_t* __restrict__ table,
+                                                                        int n_clips, int64_t total_frames, __nv_bfloat16* __restrict__ dst,
+                                                                        int h, int w) {
+    __shared__ int64_t s_off[kRaggedMaxClips];
+    __shared__ int s_first[kRaggedMaxClips + 1], s_h0[kRaggedMaxClips], s_w0[kRaggedMaxClips];
+    __shared__ float s_sy[kRaggedMaxClips], s_sx[kRaggedMaxClips];
+    pdl_sync();
+    for (int k = threadIdx.x; k < n_clips; k += blockDim.x) {
+        const int64_t* row = table + 4 * k;
+        s_off[k] = row[0];
+        s_first[k + 1] = int(row[1]);   // frame count; turned into a prefix sum below
+        s_h0[k] = int(row[2]);
+        s_w0[k] = int(row[3]);
+        s_sy[k] = float(s_h0[k]) / float(h);
+        s_sx[k] = float(s_w0[k]) / float(w);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        s_first[0] = 0;
+        for (int k = 0; k < n_clips; ++k) s_first[k + 1] += s_first[k];
+    }
+    __syncthreads();
+    const Idx total = Idx(total_frames * h * w), W = Idx(w), HW = Idx(h) * Idx(w);
+    for (Idx i = Idx(blockIdx.x) * Idx(blockDim.x) + Idx(threadIdx.x); i < total; i += Idx(gridDim.x) * Idx(blockDim.x)) {
+        const Idx fi = i / HW, r = i - fi * HW;
+        const int f = int(fi), y = int(r / W), x = int(r - (r / W) * W);
+        int lo = 0, hi = n_clips - 1;   // last clip k with s_first[k] <= f
+        while (lo < hi) {
+            const int mid = (lo + hi + 1) >> 1;
+            if (s_first[mid] <= f) lo = mid; else hi = mid - 1;
         }
-        reinterpret_cast<uint4*>(dst)[i] = pack8e(v);
+        const int H0 = s_h0[lo], W0 = s_w0[lo];
+        const uint8_t* base = src + s_off[lo] + int64_t(f - s_first[lo]) * H0 * W0 * 3;
+        reinterpret_cast<uint4*>(dst)[i] = bilinear_px8(base, H0, W0, s_sy[lo], s_sx[lo], x, y);
     }
 }
 
@@ -623,6 +673,20 @@ int t2v_frames_u8_to_nhwc8(const uint8_t* src, void* dst, int32_t F, int32_t H0,
     if (F <= 0 || H0 <= 0 || W0 <= 0 || h <= 0 || w <= 0) return fail(-2, "frames_u8_to_nhwc8: bad shape");
     launch_pdl(frames_u8_to_nhwc8_kernel, dim3(ew_grid(int64_t(F) * h * w)), dim3(256), size_t(0), ST, src, BFW(dst), F, H0, W0, h, w);
     return launch_checked(int(cudaGetLastError()), "frames_u8_to_nhwc8");
+}
+int t2v_frames_u8_to_nhwc8_ragged(const uint8_t* src, const int64_t* table, int32_t n_clips, int64_t total_frames, void* dst, int32_t h,
+                                  int32_t w, void* stream) {
+    if (n_clips <= 0 || n_clips > kRaggedMaxClips) return fail(-2, "frames_u8_to_nhwc8_ragged: %d clips (1..%d)", n_clips, kRaggedMaxClips);
+    if (total_frames < n_clips || total_frames > INT32_MAX || h <= 0 || w <= 0) return fail(-2, "frames_u8_to_nhwc8_ragged: bad shape");
+    const int64_t total = total_frames * h * w;
+    // 32-bit indices need total + the grid's stride < 2^31 (the stride is at most 16 blocks of 256 per SM)
+    if (total + int64_t(ew_grid(total)) * 256 < INT32_MAX)
+        launch_pdl(frames_u8_to_nhwc8_ragged_kernel<int32_t>, dim3(ew_grid(total)), dim3(256), size_t(0), ST, src, table, int(n_clips),
+                   total_frames, BFW(dst), int(h), int(w));
+    else
+        launch_pdl(frames_u8_to_nhwc8_ragged_kernel<int64_t>, dim3(ew_grid(total)), dim3(256), size_t(0), ST, src, table, int(n_clips),
+                   total_frames, BFW(dst), int(h), int(w));
+    return launch_checked(int(cudaGetLastError()), "frames_u8_to_nhwc8_ragged");
 }
 int t2v_gelu_bf16(const void* x, void* y, int64_t n, int32_t quick, void* stream) {
     if (n % 8) return fail(-2, "gelu: n must be a multiple of 8");

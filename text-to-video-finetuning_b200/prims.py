@@ -553,6 +553,25 @@ def frames_u8_to_nhwc8(frames, out_hw):
     return out
 
 
+def frames_u8_to_nhwc8_ragged(packed, table, out_hw):
+    """A ragged batch of clips in one launch: packed uint8 [nbytes] holds clip k's RGB frames [F_k, H0_k, W0_k, 3] at byte
+    table[k, 0]; table int64 [n, 4] = (offset, F, H0, W0) per clip -> bf16 [sum F_k, h, w, 8], clip after clip, each slice
+    bitwise equal to frames_u8_to_nhwc8 of that clip.  The table is checked against the buffer on the host (a device table
+    is read back once), then copied to the device."""
+    assert packed.dtype == torch.uint8 and packed.is_cuda and packed.is_contiguous() and packed.dim() == 1, (packed.dtype, packed.shape)
+    assert table.dtype == torch.int64 and table.dim() == 2 and table.shape[1] == 4, (table.dtype, table.shape)
+    rows = table.cpu()
+    off, F, H0, W0 = rows.unbind(1)
+    assert bool((F > 0).all() and (H0 > 0).all() and (W0 > 0).all() and (off >= 0).all()), rows
+    assert int((off + F * H0 * W0 * 3).max()) <= packed.numel(), (rows, packed.numel())
+    h, w = out_hw
+    total = int(F.sum())
+    out = torch.empty((total, h, w, 8), device=packed.device, dtype=torch.bfloat16)
+    dev_table = table.to(packed.device, non_blocking=True).contiguous()
+    native.check(native.lib().t2v_frames_u8_to_nhwc8_ragged(_p(packed), _p(dev_table), rows.shape[0], total, _p(out), h, w, _stream()))
+    return out
+
+
 def embed_tokens(ids, tok_emb, pos_emb):
     """ids int64 [B, L], tok_emb fp32 [vocab, C], pos_emb fp32 [>= L, C] -> bf16 [B*L, C] = tok_emb[ids] + pos_emb[l]."""
     assert ids.dtype == torch.int64 and ids.is_cuda and ids.is_contiguous()

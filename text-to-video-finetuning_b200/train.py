@@ -11,7 +11,9 @@ checkpoints.  One process per GPU (`torchrun --nproc-per-node N train.py --confi
 Data (SURVEY 8(f) rows 2-3): `dataset_types` in ('json', 'single_video', 'image', 'folder') build the reference's dataset
 classes (utils/dataset.py: OpenCV decode -> ONE resize + normalise kernel on the GPU -> batched AutoencoderKL.encode);
 `cache_latents: True` writes / `cached_latent_dir` reads the reference's latent cache (`cached_{i}.pt`, train.py:266-314);
-`dataset_types: ['synthetic']` needs no files.  Prompts go through the frozen CLIP text encoder (text_encoder.py) with a
+`dataset_types: ['synthetic']` needs no files.  `train_batch_size` > 1 batches items of one (frames, height, width) group
+(utils.dataset.ShapeGroupedBatches; batch size 1 keeps the plain DataLoader); with data parallelism every rank must then see
+a single group.  Prompts go through the frozen CLIP text encoder (text_encoder.py) with a
 per-prompt embedding cache; a batch that already carries `text_embeds` skips it.  `use_text_lora` (cloneofsimo only) injects
 LoRA into the text encoder (train.py:571-572) and runs it inside the step on every batch's `prompt_ids` (step.py).
 Checkpoints (8(f) row 4): LoRA in the cloneofsimo list format or the stable_lora safetensors files (full weights and the webui
@@ -129,6 +131,15 @@ class SyntheticLatents(torch.utils.data.Dataset):
     def __getitem__(self, i):
         g = torch.Generator().manual_seed(self.seed * 100003 + i)
         return {"pixel_values": torch.randn(self.shape, generator=g) * 0.18215, "text_embeds": torch.randn(self.tshape, generator=g)}
+
+
+def needs_vae(batch, latent_source):
+    """True when the batch holds pictures that still go through the VAE: raw frames (`frames_u8`, or a ragged batch packed by
+    utils.dataset.collate_raw), or `pixel_values` from a dataset of pictures.  `pixel_values` of a latent source (the cache,
+    the synthetic set) are latents.  Decided by keys and source, never by shape: a 4-frame pixel clip [B, 4, 3, h, w] and a
+    latent clip [B, 4, 3, h, w] look alike."""
+    from .utils.dataset import PACKED_KEY
+    return "frames_u8" in batch or PACKED_KEY in batch or not latent_source
 
 
 def handle_cache_latents(should_cache, output_dir, train_dataloader, vae, device, cached_latent_dir=None):
@@ -384,8 +395,19 @@ def main(
             if world > 1:
                 dist.barrier()
             dataset = CachedLatents(os.path.join(output_dir, "cached_latents"))
+    # the cache and the synthetic set hold latents; every other source holds pictures (raw frames, or pixel_values in [-1, 1]
+    # from a dataset built with device_preprocess=False) that still go through the VAE
+    latent_source = isinstance(dataset, (CachedLatents, SyntheticLatents))
     sampler = torch.utils.data.distributed.DistributedSampler(dataset, world, rank, shuffle=shuffle) if world > 1 else None
-    loader = torch.utils.data.DataLoader(dataset, batch_size=train_batch_size, shuffle=shuffle and sampler is None, sampler=sampler)
+    if train_batch_size > 1:
+        # items differ in shape (native sizes, buckets, images next to videos): batches of one shape group each
+        from .utils.dataset import ShapeGroupedBatches
+        order = sampler if sampler is not None else (
+            torch.utils.data.RandomSampler(dataset) if shuffle else torch.utils.data.SequentialSampler(dataset))
+        loader = ShapeGroupedBatches(dataset, train_batch_size, order, single_key=world > 1,
+                                     sync_device=dev if world > 1 and dist.get_backend() == "nccl" else None)
+    else:
+        loader = torch.utils.data.DataLoader(dataset, batch_size=train_batch_size, shuffle=shuffle and sampler is None, sampler=sampler)
 
     global_step, micro, epoch = 0, 0, 0
     t0 = time.time()
@@ -395,8 +417,7 @@ def main(
             sampler.set_epoch(epoch)   # a new shuffle every epoch
         epoch += 1
         for batch in loader:
-            if "frames_u8" in batch or (batch["pixel_values"].dim() == 5 and batch["pixel_values"].shape[2] == 3
-                                        and batch["pixel_values"].shape[1] != 4):
+            if needs_vae(batch, latent_source):
                 from .utils.dataset import frames_to_latents
                 latents = frames_to_latents(batch, vae, dev)        # raw clip -> resize/normalise kernel -> batched VAE encode
             else:
@@ -415,8 +436,8 @@ def main(
                                         f"({pretrained_model_path}/text_encoder is missing)")
             noise = sample_noise(latents, offset_noise_strength, use_offset_noise and not rescale_schedule)
             timesteps = torch.randint(0, abar.shape[0], (latents.shape[0],), device=dev, dtype=torch.int64)
-            if latents.shape[2] <= 1:
-                stepper.passes = 1  # single-frame data breaks out after the first pass (train.py:832)
+            # single-frame data breaks out after the first pass (train.py:832), video runs both, batch by batch
+            stepper.passes = 1 if latents.shape[2] <= 1 else 2
             loss = stepper(latents, noise, timesteps, text)   # fused: on a window boundary this includes clip + AdamW
             micro += 1
             if micro % gradient_accumulation_steps:

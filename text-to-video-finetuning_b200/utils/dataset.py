@@ -10,7 +10,10 @@ the `train_data:` section of the v2 YAML configs maps onto them unchanged.  What
     channels-last - the layout AutoencoderKL.encode consumes), see `frames_to_latents`; all frames of a clip are encoded as one
     batch (the reference encodes frame by frame with vae slicing);
   * `pixel_values` (float [F, 3, h, w] in [-1, 1], the reference's item format) is still produced - on the CPU, with the same
-    arithmetic - when a dataset is built with `device_preprocess=False` (tests, foreign consumers).
+    arithmetic - when a dataset is built with `device_preprocess=False` (tests, foreign consumers);
+  * train_batch_size > 1: `ShapeGroupedBatches` batches items of one (F, h, w) group, `collate_raw` packs clips of different
+    native sizes into one buffer, and `frames_to_latents` resizes them with ONE ragged kernel launch
+    (`prims.frames_u8_to_nhwc8_ragged`); the reference resizes on the CPU before collation instead.
 """
 import json
 import os
@@ -317,14 +320,125 @@ class CachedDataset(Dataset):
         return torch.load(self.cached_data_list[index], map_location="cpu", weights_only=False)
 
 
+# ------------------------------------------------------------------------------------------------ batches of B > 1
+PACKED_KEY, TABLE_KEY = "frames_packed", "frames_table"
+
+
+def collate_raw(items):
+    """Items of one shape group (same F, same target `pixel_hw`; native sizes may differ) -> one batch: every clip's
+    `frames_u8` back to back in ONE contiguous uint8 buffer (pinned when CUDA is present, so it crosses to the device in one
+    asynchronous copy) under `frames_packed`, and `frames_table` int64 [B, 4] = (byte offset, F, H0, W0) per clip, the
+    operands of prims.frames_u8_to_nhwc8_ragged.  `prompt_ids` and `pixel_hw` are stacked, `text_prompt` / `dataset` kept as
+    lists."""
+    hw = items[0]["pixel_hw"]
+    F = items[0]["frames_u8"].shape[0]
+    assert all(torch.equal(it["pixel_hw"], hw) for it in items), [tuple(it["pixel_hw"].tolist()) for it in items]
+    assert all(it["frames_u8"].shape[0] == F for it in items), [it["frames_u8"].shape[0] for it in items]
+    sizes = [it["frames_u8"].numel() for it in items]
+    packed = torch.empty(sum(sizes), dtype=torch.uint8, pin_memory=torch.cuda.is_available())
+    table = torch.empty((len(items), 4), dtype=torch.int64)
+    off = 0
+    for k, (it, n) in enumerate(zip(items, sizes)):
+        fr = it["frames_u8"]
+        packed[off:off + n].copy_(fr.reshape(-1))
+        table[k] = torch.tensor([off, fr.shape[0], fr.shape[1], fr.shape[2]])
+        off += n
+    batch = {PACKED_KEY: packed, TABLE_KEY: table, "pixel_hw": torch.stack([it["pixel_hw"] for it in items])}
+    for k in items[0]:
+        if k in ("frames_u8", "pixel_hw"):
+            continue
+        v = [it[k] for it in items]
+        batch[k] = torch.stack(v) if torch.is_tensor(v[0]) else v
+    return batch
+
+
+def group_key(item):
+    """What must agree across the items of one batch: (F, h, w) of the clip the step trains on.  A raw item's target size is
+    its `pixel_hw` (its native size may differ); a `pixel_values` item (pixels [F, 3, h, w] or cached latents [4, F, h, w])
+    is keyed by its exact shape, which default_collate needs equal."""
+    if "frames_u8" in item:
+        h, w = (int(v) for v in item["pixel_hw"].view(-1)[:2])
+        return ("frames", int(item["frames_u8"].shape[0]), h, w)
+    return ("pixel_values",) + tuple(item["pixel_values"].shape)
+
+
+class ShapeGroupedBatches:
+    """Batches of `batch_size` items that share one `group_key`, for train_batch_size > 1 (batch size 1 keeps the plain
+    DataLoader).  Each pass (`for batch in grouper`) is one epoch: it walks the sampler's item order, buffers every item
+    under its key and yields a batch as soon as a buffer holds `batch_size` items.  Buffers that are not full at the end of
+    an epoch carry over into the next, so no item is dropped and no batch is short (a short batch would be one more shape,
+    one more CUDA-graph capture).  The order is a pure function of the sampler's order, so a seeded sampler gives a
+    reproducible grouping.
+
+    single_key: data-parallel training (world > 1) steps every rank with the same shape, so only data with one group key
+    is supported there.  Before yielding each batch, and once at the end of each epoch, every rank joins one small
+    all-reduce of (error flag, key): a rank that meets a second key, or whose key differs from another rank's, makes EVERY
+    rank raise the same ValueError at the same point instead of leaving the others waiting in the step's collectives."""
+
+    def __init__(self, dataset, batch_size, sampler, collate=None, single_key=False, sync_device=None):
+        self.dataset, self.batch_size, self.sampler = dataset, int(batch_size), sampler
+        self.collate = collate or _collate_group
+        self.single_key, self.sync_device = single_key, sync_device
+        self.buffers = {}   # key -> items waiting for a full batch (kept across epochs)
+        self._key = None
+
+    def pending(self):
+        return sum(len(v) for v in self.buffers.values())
+
+    def __iter__(self):
+        for i in self.sampler:
+            item = self.dataset[i]
+            key = group_key(item)
+            if self.single_key:
+                if self._key is None:
+                    self._key = key
+                elif key != self._key:
+                    self._agree(f"item {i} has group key {key}, this rank's earlier items {self._key}")
+            buf = self.buffers.setdefault(key, [])
+            buf.append(item)
+            if len(buf) == self.batch_size:
+                del self.buffers[key]
+                if self.single_key:
+                    self._agree(None)
+                yield self.collate(buf)
+        if self.single_key:
+            self._agree(None)
+
+    def _agree(self, error):
+        """One all-reduce (MAX) of [error, key, -key], the key as 5 integers: the ranks' keys agree iff max == -max(-key)."""
+        import torch.distributed as dist
+        key = [0] * 5
+        if self._key is not None:
+            key = [1 + (self._key[0] == "frames")] + list(self._key[1:]) + [0] * (5 - len(self._key))
+        v = torch.tensor([1 if error else 0] + key + [-k for k in key], dtype=torch.int64, device=self.sync_device)
+        dist.all_reduce(v, op=dist.ReduceOp.MAX)
+        v = v.tolist()
+        if v[0] or v[1:6] != [-k for k in v[6:]]:
+            raise ValueError("train_batch_size > 1 with data-parallel training needs every item of every rank to share one "
+                             "(frames, height, width) group: grouping different shapes across ranks is not supported. "
+                             + (error or "another rank met a different group key") + ". Use one target size and one "
+                             "n_sample_frames (no use_bucketing, no mix of images and videos), or train_batch_size 1.")
+
+
+def _collate_group(items):
+    return collate_raw(items) if "frames_u8" in items[0] else torch.utils.data.default_collate(items)
+
+
 # ------------------------------------------------------------------------------------------------ device side
 @torch.no_grad()
-def frames_to_latents(batch, vae, device, generator=None):
+def frames_to_latents(batch, vae, device, generator=None, eps=None):
     """A collated batch of raw clips -> latents (B, 4, F, h/8, w/8) * 0.18215 on `device`: H2D of the uint8 frames, one
     resize + normalise kernel, ONE batched VAE encode of all B*F frames, fused sample / rearrange / scale kernel
-    (reference: normalize_input on the CPU, then tensor_to_vae_latent with per-frame slicing, train.py:339-347)."""
+    (reference: normalize_input on the CPU, then tensor_to_vae_latent with per-frame slicing, train.py:339-347).
+    A `collate_raw` batch (clips of different native sizes) goes through the ragged kernel in one launch.
+    eps: the sampling noise (B, 4, F, h/8, w/8); drawn from `generator` when None."""
     from .. import prims
-    if "frames_u8" in batch:
+    if PACKED_KEY in batch:
+        table = batch[TABLE_KEY]
+        B, F = table.shape[0], int(table[0, 1])
+        hw = tuple(int(v) for v in batch["pixel_hw"].view(-1, 2)[0])
+        nhwc8 = prims.frames_u8_to_nhwc8_ragged(batch[PACKED_KEY].to(device, non_blocking=True), table, hw)
+    elif "frames_u8" in batch:
         fr = batch["frames_u8"]                       # [B, F, H0, W0, 3] uint8
         B, F = fr.shape[:2]
         hw = tuple(int(v) for v in batch["pixel_hw"].view(-1, 2)[0])
@@ -336,8 +450,9 @@ def frames_to_latents(batch, vae, device, generator=None):
         nhwc8 = prims.latents_to_nhwc8(pv.reshape(B * F, 3, 1, pv.shape[-2], pv.shape[-1]).contiguous())
     mom = vae.encode_moments_nhwc8(nhwc8)
     _, h, w, _ = mom.shape
-    eps = torch.randn((B, 4, F, h, w), device=mom.device, dtype=torch.float32, generator=generator)
-    return prims.vae_sample(mom, eps, B, F, 0.18215)
+    if eps is None:
+        eps = torch.randn((B, 4, F, h, w), device=mom.device, dtype=torch.float32, generator=generator)
+    return prims.vae_sample(mom, eps.to(mom.device, torch.float32).contiguous(), B, F, 0.18215)
 
 
 DATASETS = {cls.__getname__(): cls for cls in (VideoJsonDataset, SingleVideoDataset, ImageDataset, VideoFolderDataset)}
