@@ -68,11 +68,13 @@ struct GnArgs {
 };
 
 enum { GN_FWD_APPLY = 0, GN_BWD_SUMS = 1, GN_BWD_APPLY = 2, GN_FWD_SUMS = 3 };
+constexpr int GN_CSLOTS = 8;   // channels per thread in the statistics prologue: C / blockDim.x <= 8 (gn_stream)
 
 template <int MODE>
-__global__ void __launch_bounds__(384, 2) gn_stream_kernel(const GnArgs g) {
+__global__ void __launch_bounds__(384, MODE == GN_BWD_SUMS ? 1 : 2) gn_stream_kernel(const GnArgs g) {
     pdl_sync();
-    extern __shared__ float sh[];  // [2][C] per-channel sums, then [2][G] group terms
+    extern __shared__ float sh[];  // apply: [2][C] per-channel sums, [2][G] group terms (bwd: + [C] gamma, [G] float2 stat);
+                                   // sums: [4][blockDim] float4
     constexpr bool kSums = MODE == GN_BWD_SUMS || MODE == GN_FWD_SUMS;
     constexpr bool kBwd = MODE == GN_BWD_SUMS || MODE == GN_BWD_APPLY;
     const int C = g.C, G = g.G, cpg = C / G;
@@ -90,17 +92,24 @@ __global__ void __launch_bounds__(384, 2) gn_stream_kernel(const GnArgs g) {
     float* cs = sh;              // [2][C]
     float* t0 = sh + 2 * C;      // [G]  fwd: group mean   bwd: sum_c gamma * sum dz
     float* t1 = t0 + G;          // [G]  fwd: group rstd   bwd: sum_c gamma * sum dz*xhat
+    float* gs = t1 + G;          // [C]  bwd: gamma
+    float2* ss = reinterpret_cast<float2*>(gs + C);   // [G] bwd apply: (mean, rstd)
     float a[8], b[8], gam[8];
 
-    // backward modes: saved per-channel coefficients (independent of the prologue below: fetched ahead of it)
+    // backward modes: saved per-channel coefficients.  The sums pass needs them first; the apply pass fetches (a, b) after
+    // the statistics loads, so that they land during the group combine instead of holding registers across the prologue, and
+    // reads (mean, rstd) from shared memory, where the prologue put them
     float mean[8], rstd[8];
-    if (kBwd) {
+    auto load_ab = [&]() {
         const float4* ab4 = reinterpret_cast<const float4*>(g.ab + (int64_t(s) * C + cv * 8) * 2);
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             const float4 q = __ldg(ab4 + j);
             a[2 * j] = q.x; b[2 * j] = q.y; a[2 * j + 1] = q.z; b[2 * j + 1] = q.w;
         }
+    };
+    if (MODE == GN_BWD_SUMS) {
+        load_ab();
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
             const int c = cv * 8 + j;
@@ -109,7 +118,7 @@ __global__ void __launch_bounds__(384, 2) gn_stream_kernel(const GnArgs g) {
         }
     }
     // apply modes: this thread's first pixels do not depend on the statistics - their loads are issued now and land while the
-    // block finalises its sample's statistics (two dependent L2 round trips and two barriers)
+    // block finalises its sample's statistics (one L2 round trip and two barriers)
     constexpr int UA = MODE == GN_FWD_APPLY ? 4 : 2;
     uint4 fx[UA], fd[UA];
     if (!kSums) {
@@ -126,55 +135,91 @@ __global__ void __launch_bounds__(384, 2) gn_stream_kernel(const GnArgs g) {
 
     if (!kSums) {
         // ---- finalise this sample's statistics (redundantly per block: C values from L2, one round trip)
-#pragma unroll
-        for (int j = 0; j < 8; ++j) gam[j] = __ldg(g.gamma + cv * 8 + j);
+        // blockDim.x = V * lanes >= C / 8, so a thread owns at most GN_CSLOTS of the C channels: all its loads are issued
+        // before the first use, one L2 round trip instead of one per channel slot
         if (MODE == GN_FWD_APPLY) {
+            float2 sum[GN_CSLOTS];
 #pragma unroll
-            for (int j = 0; j < 8; ++j) b[j] = __ldg(g.beta + cv * 8 + j);
-            for (int c = threadIdx.x; c < C; c += blockDim.x) {
-                const bool first = c < g.C0;
-                const float2* src = reinterpret_cast<const float2*>(first ? g.stats0 : g.stats1) + (first ? c : c - g.C0);
-                const int64_t ld = first ? g.ld0 : g.ld1;
-                float a0 = 0.f, a1 = 0.f;
-#pragma unroll 4
-                for (int f = 0; f < g.fps; ++f) {   // a few slots per sample (layers.clip_stats_rows): independent loads
-                    const float2 v = __ldcg(src + (int64_t(s) * g.fps + f) * ld);
-                    a0 += v.x;
-                    a1 += v.y;
+            for (int i = 0; i < GN_CSLOTS; ++i) sum[i] = make_float2(0.f, 0.f);
+            for (int f = 0; f < g.fps; ++f) {   // a few slots per sample (layers.clip_stats_rows)
+#pragma unroll
+                for (int i = 0; i < GN_CSLOTS; ++i) {
+                    const int c = threadIdx.x + i * blockDim.x;
+                    if (c < C) {
+                        const bool first = c < g.C0;
+                        const float2* src = reinterpret_cast<const float2*>(first ? g.stats0 : g.stats1) + (first ? c : c - g.C0);
+                        const float2 v = __ldcg(src + (int64_t(s) * g.fps + f) * (first ? g.ld0 : g.ld1));
+                        sum[i].x += v.x;
+                        sum[i].y += v.y;
+                    }
                 }
-                cs[c] = a0;
-                cs[C + c] = a1;
+            }
+#pragma unroll
+            for (int i = 0; i < GN_CSLOTS; ++i) {
+                const int c = threadIdx.x + i * blockDim.x;
+                if (c < C) {
+                    cs[c] = sum[i].x;
+                    cs[C + c] = sum[i].y;
+                }
             }
         } else {
             const float2* acc = reinterpret_cast<const float2*>(g.accum + int64_t(s) * C * 2);
-            for (int c = threadIdx.x; c < C; c += blockDim.x) {
-                const float2 v = __ldcg(acc + c);
-                cs[c] = v.x;
-                cs[C + c] = v.y;
-                if (chunk == 0) {
-                    if (g.dbeta) atomicAdd(g.dbeta + c, v.x);
-                    if (g.dgamma) atomicAdd(g.dgamma + c, v.y);
+            float2 v[GN_CSLOTS], ms[GN_CSLOTS];
+            float w[GN_CSLOTS];
+#pragma unroll
+            for (int i = 0; i < GN_CSLOTS; ++i) {
+                const int c = threadIdx.x + i * blockDim.x;
+                if (c < C) {
+                    v[i] = __ldcg(acc + c);
+                    w[i] = __ldg(g.gamma + c);
+                    if (c < G) ms[i] = __ldg(reinterpret_cast<const float2*>(g.stat) + int64_t(s) * G + c);
+                }
+            }
+#pragma unroll
+            for (int i = 0; i < GN_CSLOTS; ++i) {
+                const int c = threadIdx.x + i * blockDim.x;
+                if (c < C) {
+                    cs[c] = v[i].x;
+                    cs[C + c] = v[i].y;
+                    gs[c] = w[i];
+                    if (c < G) ss[c] = ms[i];
+                    if (chunk == 0) {
+                        if (g.dbeta) atomicAdd(g.dbeta + c, v[i].x);
+                        if (g.dgamma) atomicAdd(g.dgamma + c, v[i].y);
+                    }
                 }
             }
         }
         __syncthreads();
-        {   // full warps only: one warp per group, fp64 combine of the group's channels through shuffles
+        if (MODE == GN_FWD_APPLY) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                gam[j] = __ldg(g.gamma + cv * 8 + j);
+                b[j] = __ldg(g.beta + cv * 8 + j);
+            }
+        } else {
+            load_ab();
+        }
+        {   // full warps only: four lanes per group, eight groups per warp at a time, fp64 combine through shuffles
             const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
             if (warp < nw) {
-                for (int gi = warp; gi < G; gi += nw) {
+                for (int g8 = warp * 8; g8 < G; g8 += nw * 8) {
+                    const int gi = g8 + (lane >> 2);
                     double a0 = 0, a1 = 0;
-                    for (int j = lane; j < cpg; j += 32) {
-                        const int c = gi * cpg + j;
-                        const double w = MODE == GN_FWD_APPLY ? 1.0 : double(__ldg(g.gamma + c));
-                        a0 += w * cs[c];
-                        a1 += w * cs[C + c];
+                    if (gi < G) {
+                        for (int j = lane & 3; j < cpg; j += 4) {
+                            const int c = gi * cpg + j;
+                            const double w = MODE == GN_FWD_APPLY ? 1.0 : double(gs[c]);
+                            a0 += w * cs[c];
+                            a1 += w * cs[C + c];
+                        }
                     }
 #pragma unroll
-                    for (int o = 16; o > 0; o >>= 1) {
+                    for (int o = 1; o < 4; o <<= 1) {
                         a0 += __shfl_xor_sync(0xffffffffu, a0, o);
                         a1 += __shfl_xor_sync(0xffffffffu, a1, o);
                     }
-                    if (lane == 0) {
+                    if (gi < G && (lane & 3) == 0) {
                         if (MODE == GN_FWD_APPLY) {
                             const double n = double(g.P) * cpg;
                             const double m = a0 / n;
@@ -237,8 +282,6 @@ __global__ void __launch_bounds__(384, 2) gn_stream_kernel(const GnArgs g) {
     }
 
     if (kSums) {
-        for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) sh[i] = 0.f;
-        __syncthreads();
         float acc0[8], acc1[8];
 #pragma unroll
         for (int j = 0; j < 8; ++j) acc0[j] = acc1[j] = 0.f;
@@ -281,22 +324,25 @@ __global__ void __launch_bounds__(384, 2) gn_stream_kernel(const GnArgs g) {
             for (int u = 0; u < U; ++u)
                 if (p + u * lanes < np) accumulate(qx[u], qd[u]);
         }
-        if (lanes == 1) {   // one pixel lane per channel vector: no contention, plain stores
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                sh[cv * 8 + j] = acc0[j];
-                sh[C + cv * 8 + j] = acc1[j];
-            }
-        } else {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                atomicAdd(&sh[cv * 8 + j], acc0[j]);
-                atomicAdd(&sh[C + cv * 8 + j], acc1[j]);
-            }
-        }
+        // Per-block reduction over the pixel lanes without shared-memory atomics (a float atomicAdd on shared memory is a CAS
+        // loop on sm_90): every thread stages its 16 partials as [4][blockDim] float4, then one thread per channel sums
+        // them over the lanes in lane order and issues one red.add.
+        float4* st = reinterpret_cast<float4*>(sh) + threadIdx.x;
+        st[0] = make_float4(acc0[0], acc0[1], acc0[2], acc0[3]);
+        st[blockDim.x] = make_float4(acc0[4], acc0[5], acc0[6], acc0[7]);
+        st[2 * blockDim.x] = make_float4(acc1[0], acc1[1], acc1[2], acc1[3]);
+        st[3 * blockDim.x] = make_float4(acc1[4], acc1[5], acc1[6], acc1[7]);
         __syncthreads();
         float* acc = g.accum + int64_t(s) * C * 2;
-        for (int c = threadIdx.x; c < C; c += blockDim.x) red_add_f32x2(acc + 2 * c, sh[c], sh[C + c]);
+        for (int c = threadIdx.x; c < C; c += blockDim.x) {
+            const float* col = sh + ((c & 4) ? blockDim.x * 4 : 0) + (c >> 3) * 4 + (c & 3);   // float4 q = (c & 7) / 4, vector c / 8
+            float s0 = 0.f, s1 = 0.f;
+            for (int l = 0; l < lanes; ++l) {
+                s0 += col[l * V * 4];
+                s1 += col[l * V * 4 + blockDim.x * 8];
+            }
+            red_add_f32x2(acc + 2 * c, s0, s1);
+        }
         return;
     }
 
@@ -306,18 +352,18 @@ __global__ void __launch_bounds__(384, 2) gn_stream_kernel(const GnArgs g) {
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
         const int c = cv * 8 + j;
-        const float q = -rstd[j] * rstd[j] * t1[c / cpg] * invn;
-        pc[j] = rstd[j] * gam[j];
+        const float m = ss[c / cpg].x, r = ss[c / cpg].y;
+        const float q = -r * r * t1[c / cpg] * invn;
+        pc[j] = r * gs[c];
         qc[j] = q;
-        rc[j] = -rstd[j] * t0[c / cpg] * invn - q * mean[j];
+        rc[j] = -r * t0[c / cpg] * invn - q * m;
     }
     uint4* os = reinterpret_cast<uint4*>(g.out) + base;
     const uint4* as = g.add ? reinterpret_cast<const uint4*>(g.add) + base : nullptr;
-    auto apply = [&](const uint4& qx, const uint4& qd, const uint4& qa) {
-        float v[8], d[8], r[8];
+    auto apply = [&](const uint4& qx, const uint4& qd, float* v) {
+        float d[8];
         unpack8(qx, v);
         unpack8(qd, d);
-        unpack8(qa, r);
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
             float dz = d[j];
@@ -326,27 +372,51 @@ __global__ void __launch_bounds__(384, 2) gn_stream_kernel(const GnArgs g) {
                 const float sg = sigmoidf_(z);
                 dz *= sg * (1.f + z * (1.f - sg));
             }
-            v[j] = pc[j] * dz + qc[j] * v[j] + rc[j] + r[j];
+            v[j] = pc[j] * dz + qc[j] * v[j] + rc[j];
         }
+    };
+    auto apply_add = [&](const uint4& qx, const uint4& qd, const uint4& qa) {
+        float v[8], r[8];
+        apply(qx, qd, v);
+        unpack8(qa, r);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) v[j] += r[j];
         return pack8(v);
     };
-    const uint4 zero = make_uint4(0, 0, 0, 0);
 #pragma unroll
-    for (int u = 0; u < 2; ++u)
-        if (pl + u * lanes < np) os[(pl + u * lanes) * V] = apply(fx[u], fd[u], as ? __ldg(as + (pl + u * lanes) * V) : zero);
+    for (int u = 0; u < 2; ++u) {
+        if (pl + u * lanes < np) {
+            float v[8];
+            if (as) {
+                os[(pl + u * lanes) * V] = apply_add(fx[u], fd[u], __ldg(as + (pl + u * lanes) * V));
+            } else {
+                apply(fx[u], fd[u], v);
+                os[(pl + u * lanes) * V] = pack8(v);
+            }
+        }
+    }
+    if (as) {   // residual gradient: one pixel (three vectors) in flight, which keeps the 80-register budget of the bound
+        for (int p = pl + 2 * lanes, off = p * V; p < np; p += lanes, off += stepv)
+            os[off] = apply_add(__ldg(xs + off), __ldg(ds + off), __ldg(as + off));
+        return;
+    }
     for (int p = pl + 2 * lanes, off = p * V; p < np; p += 2 * lanes, off += 2 * stepv) {
-        uint4 qx[2], qd[2], qa[2];
+        uint4 qx[2], qd[2];
 #pragma unroll
         for (int u = 0; u < 2; ++u) {
             if (p + u * lanes < np) {
                 qx[u] = __ldg(xs + off + u * stepv);
                 qd[u] = __ldg(ds + off + u * stepv);
-                qa[u] = as ? __ldg(as + off + u * stepv) : zero;
             }
         }
 #pragma unroll
-        for (int u = 0; u < 2; ++u)
-            if (p + u * lanes < np) os[off + u * stepv] = apply(qx[u], qd[u], qa[u]);
+        for (int u = 0; u < 2; ++u) {
+            if (p + u * lanes < np) {
+                float v[8];
+                apply(qx[u], qd[u], v);
+                os[off + u * stepv] = pack8(v);
+            }
+        }
     }
 }
 
@@ -420,8 +490,11 @@ __global__ void ln_fwd_kernel(const __nv_bfloat16* __restrict__ x, const float* 
 // Register budget: the per-lane parameter-gradient accumulators (16 VPL floats) are the only fp32 arrays that live across rows;
 // the row itself stays packed (bf16, as loaded) and is unpacked twice - once for the row sums, once for dx - and gamma comes
 // from L1 each time, so two 256-thread blocks stay resident per SM up to C = 640.
+constexpr int LN_BWD_WARPS = 8;   // 256-thread blocks
+constexpr size_t LN_BWD_SMEM = LN_BWD_WARPS * 4 * 32 * sizeof(float4);
+
 template <int VPL>
-__global__ void __launch_bounds__(256, VPL <= 3 ? 2 : 1) ln_bwd_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ dy,
+__global__ void __launch_bounds__(LN_BWD_WARPS * 32, VPL <= 3 ? 2 : 1) ln_bwd_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ dy,
                               const float* __restrict__ gamma, const float* __restrict__ stat,
                               const __nv_bfloat16* __restrict__ add, __nv_bfloat16* __restrict__ dx,
                               float* __restrict__ dgamma, float* __restrict__ dbeta, int64_t rows, int C) {
@@ -436,7 +509,10 @@ __global__ void __launch_bounds__(256, VPL <= 3 ? 2 : 1) ln_bwd_kernel(const __n
 #pragma unroll
         for (int j = 0; j < 8; ++j) gacc[k][j] = bacc[k][j] = 0.f;
     // software pipeline over this warp's rows: x, dy and the saved statistics of the next row are in flight while the
-    // current row is reduced; the residual-gradient vector (`add`) of the current row is fetched ahead of the reductions
+    // current row is reduced.  The dx pass takes the current row from a register copy where that copy fits the launch
+    // bound's register budget next to the 16 VPL accumulators (128 registers for VPL <= 3, 255 above), and otherwise
+    // re-reads it (L1 hits: the warp has just loaded it); ptxas -v shows no spills either way.
+    constexpr bool kHold = VPL <= 2 || (VPL >= 4 && VPL <= 5);
     uint4 nx[VPL], nd[VPL];
     float2 nst = make_float2(0.f, 0.f);
     auto fetch = [&](int64_t row) {
@@ -452,18 +528,19 @@ __global__ void __launch_bounds__(256, VPL <= 3 ? 2 : 1) ln_bwd_kernel(const __n
     if (warp < rows) fetch(warp);
     for (int64_t row = warp; row < rows; row += nwarps) {
         const float mean = nst.x, rstd = nst.y;
-        uint4 cx[VPL], cd[VPL], ra[VPL];
+        uint4 cx[kHold ? VPL : 1], cd[kHold ? VPL : 1];
         float s1 = 0.f, s2 = 0.f;
 #pragma unroll
         for (int k = 0; k < VPL; ++k) {
             const int cv = lane + 32 * k;
             if (cv < V) {
-                cx[k] = nx[k];
-                cd[k] = nd[k];
-                if (add) ra[k] = __ldg(reinterpret_cast<const uint4*>(add + row * C) + cv);
+                if (kHold) {
+                    cx[k] = nx[k];
+                    cd[k] = nd[k];
+                }
                 float v[8], d[8];
-                unpack8(cx[k], v);
-                unpack8(cd[k], d);
+                unpack8(nx[k], v);
+                unpack8(nd[k], d);
                 const float4 g0 = __ldg(reinterpret_cast<const float4*>(gamma) + cv * 2), g1 = __ldg(reinterpret_cast<const float4*>(gamma) + cv * 2 + 1);
                 const float gm[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
 #pragma unroll
@@ -490,9 +567,9 @@ __global__ void __launch_bounds__(256, VPL <= 3 ? 2 : 1) ln_bwd_kernel(const __n
             const int cv = lane + 32 * k;
             if (cv < V) {
                 float v[8], d[8], o[8], r[8];
-                unpack8(cx[k], v);
-                unpack8(cd[k], d);
-                if (add) unpack8(ra[k], r);
+                unpack8(kHold ? cx[k] : __ldg(reinterpret_cast<const uint4*>(x + row * C) + cv), v);
+                unpack8(kHold ? cd[k] : __ldg(reinterpret_cast<const uint4*>(dy + row * C) + cv), d);
+                if (add) unpack8(__ldg(reinterpret_cast<const uint4*>(add + row * C) + cv), r);
                 const float4 g0 = __ldg(reinterpret_cast<const float4*>(gamma) + cv * 2), g1 = __ldg(reinterpret_cast<const float4*>(gamma) + cv * 2 + 1);
                 const float gm[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
 #pragma unroll
@@ -505,29 +582,42 @@ __global__ void __launch_bounds__(256, VPL <= 3 ? 2 : 1) ln_bwd_kernel(const __n
             }
         }
     }
-    // block-level reduction of the parameter gradients, then one atomic per channel per block
-    extern __shared__ float sh[];  // [2][C]
-    for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) sh[i] = 0.f;
-    __syncthreads();
+    // Block-level reduction of the parameter gradients, then one red.add per channel per block.  No shared-memory atomics:
+    // a float atomicAdd on shared memory is a CAS loop on sm_90, and eight warps contending for the same 2C words cost more
+    // than the rows themselves.  Per 32-channel-vector slice k, every warp stages its 16 partials per lane ([q][lane] float4,
+    // conflict-free), then each thread sums one gamma and one beta partial over the eight warps in warp order.
+    extern __shared__ float4 stage[];  // [LN_BWD_WARPS][4][32]
+    const int wib = threadIdx.x >> 5;
+    const int t = threadIdx.x, rl = (t >> 2) & 31, rc = (t >> 7) * 4 + (t & 3);   // reader: lane, channel within the vector
 #pragma unroll
     for (int k = 0; k < VPL; ++k) {
-        const int cv = lane + 32 * k;
-        if (cv < V) {
+        if (k) __syncthreads();
+        float4* st = stage + wib * 128 + lane;
+        st[0] = make_float4(gacc[k][0], gacc[k][1], gacc[k][2], gacc[k][3]);
+        st[32] = make_float4(gacc[k][4], gacc[k][5], gacc[k][6], gacc[k][7]);
+        st[64] = make_float4(bacc[k][0], bacc[k][1], bacc[k][2], bacc[k][3]);
+        st[96] = make_float4(bacc[k][4], bacc[k][5], bacc[k][6], bacc[k][7]);
+        __syncthreads();
+        if (rl + 32 * k < V) {
+            const float* sf = reinterpret_cast<const float*>(stage);
+            float sg = 0.f, sb = 0.f;
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                atomicAdd(&sh[cv * 8 + j], gacc[k][j]);
-                atomicAdd(&sh[C + cv * 8 + j], bacc[k][j]);
+            for (int w = 0; w < LN_BWD_WARPS; ++w) {
+                sg += sf[w * 512 + t];
+                sb += sf[w * 512 + 256 + t];
             }
+            const int c = (rl + 32 * k) * 8 + rc;
+            if (dgamma) atomicAdd(dgamma + c, sg);
+            if (dbeta) atomicAdd(dbeta + c, sb);
         }
-    }
-    __syncthreads();
-    for (int c = threadIdx.x; c < C; c += blockDim.x) {
-        if (dgamma) atomicAdd(dgamma + c, sh[c]);
-        if (dbeta) atomicAdd(dbeta + c, sh[C + c]);
     }
 }
 
-static size_t gn_smem(int C, int G) { return size_t(2 * C + 2 * G) * sizeof(float); }
+// dynamic shared memory of gn_stream_kernel<MODE> (layout at its declaration of sh)
+static size_t gn_smem(int mode, int C, int G, int threads) {
+    if (mode == GN_BWD_SUMS || mode == GN_FWD_SUMS) return size_t(threads) * 4 * sizeof(float4);
+    return size_t(2 * C + 2 * G + (mode == GN_BWD_APPLY ? C + 2 * G : 0)) * sizeof(float);
+}
 
 // Streaming geometry: threads = V * lanes (<= 256, or V itself up to 384 for the 2560- / 3072-channel concatenations), a
 // block owns `chunk_pixels` pixels of one sample.  Apply modes: exactly ONE wave of blocks - as many as are resident at once
@@ -547,7 +637,7 @@ static void gn_plan(GnArgs& g, int S, bool sums, int resident) {
 }
 
 static int gn_check(const GnArgs& g) {
-    if (g.C % 8 || g.C % g.G || g.C / 8 > 384 || gn_smem(g.C, g.G) > 48 * 1024)
+    if (g.C % 8 || g.C % g.G || g.C / 8 > 384 || gn_smem(GN_BWD_APPLY, g.C, g.G, 0) > 48 * 1024)
         return fail(-2, "groupnorm: C=%d G=%d unsupported", g.C, g.G);
     return 0;
 }
@@ -572,8 +662,9 @@ static int gn_stream(GnArgs& g, int S, cudaStream_t st) {
     const bool sums = MODE == GN_BWD_SUMS || MODE == GN_FWD_SUMS;
     const int V = g.C / 8;
     const int threads = V * std::max(1, 256 / V);
-    gn_plan(g, S, sums, sums ? 0 : gn_resident<MODE>(threads, gn_smem(g.C, g.G)));
-    return int(launch_pdl(gn_stream_kernel<MODE>, dim3(S * g.chunks), dim3(V * g.lanes), gn_smem(g.C, g.G), st, g));
+    const size_t smem = gn_smem(MODE, g.C, g.G, threads);
+    gn_plan(g, S, sums, sums ? 0 : gn_resident<MODE>(threads, smem));
+    return int(launch_pdl(gn_stream_kernel<MODE>, dim3(S * g.chunks), dim3(V * g.lanes), smem, st, g));
 }
 
 // Standalone per-sample channel sums of x [S][P][C] into stats (+=), row pitch ld channels.  Used by t2v_channel_stats and
@@ -702,8 +793,8 @@ int t2v_layernorm_bwd(const void* dy, const void* x, const float* gamma, const f
     if (C % 8 || C > 2048) return fail(-2, "layernorm: C=%d unsupported (multiple of 8, <= 2048)", C);
     cudaStream_t st = static_cast<cudaStream_t>(stream_);
     const int vpl = (C / 8 + 31) / 32;
-    const int grid = int(std::min<int64_t>((rows + 7) / 8, int64_t(device_sm_count()) * ln_resident(true, vpl, 2 * C * sizeof(float))));
-    LN_DISPATCH(ln_bwd_kernel, grid, 2 * C * sizeof(float), st, static_cast<const __nv_bfloat16*>(x),
+    const int grid = int(std::min<int64_t>((rows + 7) / 8, int64_t(device_sm_count()) * ln_resident(true, vpl, LN_BWD_SMEM)));
+    LN_DISPATCH(ln_bwd_kernel, grid, LN_BWD_SMEM, st, static_cast<const __nv_bfloat16*>(x),
                 static_cast<const __nv_bfloat16*>(dy), gamma, stat, static_cast<const __nv_bfloat16*>(add),
                 static_cast<__nv_bfloat16*>(dx), dgamma, dbeta, rows, C);
     return launch_checked(int(cudaGetLastError()), "layernorm_bwd");
