@@ -188,18 +188,27 @@ class FusedAdamW(torch.optim.Optimizer):
     # ------------------------------------------------------------------------------------------------ step
     def push_hyperparams(self):
         """Host -> device copy of (lr, beta1, beta2, eps, weight_decay) per set (stream-ordered, before the step's kernels or
-        the graph replay).  A scheduler that makes groups of one set diverge triggers a rebuild of the tables."""
-        for s in self._sets:
-            if any(self._key(self.param_groups[gi])[1:] != s["key"][1:] or
-                   self.param_groups[gi]["lr"] != self.param_groups[s["groups"][0]]["lr"] for gi in s["groups"]):
-                self._build()
-                break
+        the graph replay).  A scheduler that makes groups of one set diverge triggers a rebuild of the tables.  The check runs
+        only when some group's hyper-parameters differ from the previous call's (a run with one group per tensor has
+        ~1,500 groups, and this is host time on every optimizer step)."""
+        seen = [(g["lr"], tuple(g["betas"]), g["eps"], g["weight_decay"]) for g in self.param_groups]
+        if seen != getattr(self, "_hp_seen", None):
+            self._check_sets()
+            self._hp_seen = seen
         for i, s in enumerate(self._sets):
             g = self.param_groups[s["groups"][0]]
             self.hp_host[i, 0] = float(g["lr"])
             self.hp_host[i, 1], self.hp_host[i, 2] = float(g["betas"][0]), float(g["betas"][1])
             self.hp_host[i, 3], self.hp_host[i, 4] = float(g["eps"]), float(g["weight_decay"])
         self.hp_in.copy_(self.hp_host, non_blocking=True)
+
+    def _check_sets(self):
+        """Rebuild the tables when the groups of one set no longer share their hyper-parameters."""
+        for s in self._sets:
+            if any(self._key(self.param_groups[gi])[1:] != s["key"][1:] or
+                   self.param_groups[gi]["lr"] != self.param_groups[s["groups"][0]]["lr"] for gi in s["groups"]):
+                self._build()
+                break
 
     def launch(self, zero_grad=True, grad_bf16=None):
         """The device-only part of one step (capturable): gradient norm, scalars, update.  grad_bf16: flat bf16 twin of the

@@ -109,12 +109,17 @@ class ParamArena:
 
     def reattach_grads(self):
         """optimizer.zero_grad(set_to_none=True) drops the views; put them back (trainable parameters only: a frozen
-        parameter's grad stays None, which is what makes torch optimizers skip it - no weight decay on frozen weights)."""
+        parameter's grad stays None, which is what makes torch optimizers skip it - no weight decay on frozen weights).
+        Runs before every step: when every parameter still holds the gradient object set here last time, nothing is done."""
+        views = getattr(self, "_grad_views", None)
+        if views is not None and all(p.grad is v for p, v in zip(self.params, views)):
+            return
         for p, o in zip(self.params, self.offsets):
             if not p.requires_grad:
                 p.grad = None
             elif p.grad is None or p.grad.data_ptr() != self.grad.data_ptr() + 4 * o:
                 p.grad = torch.as_strided(self.grad, p.shape, p.stride(), o)
+        self._grad_views = [p.grad for p in self.params]
 
     def grad_norm(self):
         return self.grad.norm()

@@ -147,6 +147,11 @@ class DataParallelStep:
         self.accumulation = max(1, int(accumulation))
         self._micro = 0
         self._graphs = {}
+        # A capture draws the dropout host seeds from torch's CPU generator (twice in warm-up, once in the capture) and the
+        # graph keeps the last ones.  capture_rng: graph key (without the optimizer generation) -> the CPU generator state at
+        # the start of its capture.  replay_rng: states a resumed run captures those keys from, so its graphs hold the seeds
+        # of the run it continues (train.py, save_training_state).
+        self.capture_rng, self.replay_rng = {}, {}
         self._gscale = None
         # world > 1: per-block gradient all-reduces are issued from inside the backward pass (overlap), see GradientBuckets
         self.buckets = None
@@ -158,6 +163,7 @@ class DataParallelStep:
     def attach_optimizer(self, optimizer):
         self.optimizer = optimizer
         self._graphs = {}
+        self.capture_rng = {}
 
     def _fwd_bwd(self, latents, noise, timesteps, text, first, last):
         """first / last: position of this micro-step inside its accumulation window."""
@@ -220,9 +226,18 @@ class DataParallelStep:
                    tuple(tuple(a.shape) for a in args))
             g = self._graphs.get(key)
             if g is None:
+                seeds_key = key[:4] + key[5:]
+                recorded = self.replay_rng.pop(seeds_key, None)
+                live = None
+                if recorded is not None:   # draw the seeds the interrupted run drew, then give the live stream back
+                    live = torch.get_rng_state()
+                    torch.set_rng_state(recorded)
+                self.capture_rng[seeds_key] = torch.get_rng_state()
                 # the capture runs the step for real (warm-up + capture replays nothing): keep the optimizer state and the
                 # weights of those dry runs out of the training trajectory
                 g = self._graphs[key] = GraphedStep(lambda *a: self._fwd_bwd(*a, first, last), args, snapshot=self._snapshot())
+                if live is not None:
+                    torch.set_rng_state(live)
             return g(*args)
         return self._fwd_bwd(*args, first, last)
 

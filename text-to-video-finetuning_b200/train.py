@@ -248,6 +248,7 @@ def main(
     lora_unet_dropout: float = 0.1,
     lora_text_dropout: float = 0.1,
     logger_type: str = "tensorboard",
+    save_training_state: bool = False,
     **kwargs,
 ):
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -399,24 +400,62 @@ def main(
     # from a dataset built with device_preprocess=False) that still go through the VAE
     latent_source = isinstance(dataset, (CachedLatents, SyntheticLatents))
     sampler = torch.utils.data.distributed.DistributedSampler(dataset, world, rank, shuffle=shuffle) if world > 1 else None
+    # the epoch's item order and position, recorded for a resume; the order is the plain sampler's
+    from .utils.dataset import EpochOrder
+    order = EpochOrder(sampler if sampler is not None else (
+        torch.utils.data.RandomSampler(dataset) if shuffle else torch.utils.data.SequentialSampler(dataset)))
     if train_batch_size > 1:
         # items differ in shape (native sizes, buckets, images next to videos): batches of one shape group each
         from .utils.dataset import ShapeGroupedBatches
-        order = sampler if sampler is not None else (
-            torch.utils.data.RandomSampler(dataset) if shuffle else torch.utils.data.SequentialSampler(dataset))
         loader = ShapeGroupedBatches(dataset, train_batch_size, order, single_key=world > 1,
                                      sync_device=dev if world > 1 and dist.get_backend() == "nccl" else None)
     else:
-        loader = torch.utils.data.DataLoader(dataset, batch_size=train_batch_size, shuffle=shuffle and sampler is None, sampler=sampler)
+        loader = torch.utils.data.DataLoader(dataset, batch_size=train_batch_size, sampler=order)
 
     global_step, micro, epoch = 0, 0, 0
+    from . import training_state as TS
+
+    def state_manifest():
+        return TS.manifest(world, lora_version, optimizer, use_ema, stepper, global_step, epoch)
+
+    def save_state(path):
+        TS.save(path, rank=rank, world=world, man=state_manifest(), stepper=stepper, optimizer=optimizer, sched=sched,
+                order=order, loader=loader)
+
+    resume_rng, skip_batches = None, 0
+    target = _resume_target(resume_from_checkpoint, output_dir)
+    if target is not None:
+        state_dir = os.path.join(target, TS.STATE_DIR)
+        if TS.is_complete(state_dir):
+            saved = TS.read_manifest(state_dir)
+            TS.check(saved, state_manifest())
+            resume_rng = TS.load(state_dir, rank=rank, stepper=stepper, optimizer=optimizer, sched=sched, order=order, loader=loader)
+            global_step = int(saved["global_step"])
+            epoch = int(saved["epoch"]) - 1   # the loop below re-enters the saved epoch
+            micro = stepper._micro = global_step * gradient_accumulation_steps
+            if rank == 0:
+                print(f"resumed from {state_dir} at step {global_step}")
+        elif resume_step is not None:
+            # the reference's resume (train.py:842-846): skip the first resume_step batches of the first epoch, load nothing
+            skip_batches = int(resume_step)
+        else:
+            raise ValueError(f"resume_from_checkpoint={resume_from_checkpoint!r}: {state_dir} holds no complete training state; "
+                             "train with save_training_state: True to write one next to every checkpoint (or give resume_step "
+                             "to only skip batches, as the reference does)")
     t0 = time.time()
     step_times, t_iter = [], time.perf_counter()
     while global_step < max_train_steps:
         if sampler is not None:
             sampler.set_epoch(epoch)   # a new shuffle every epoch
         epoch += 1
-        for batch in loader:
+        batches = iter(loader)
+        if resume_rng is not None:   # after the iterator's own draw, which the uninterrupted run made before the checkpoint
+            TS.restore_rng(resume_rng, dev)
+            resume_rng = None
+        for batch in batches:
+            if skip_batches:
+                skip_batches -= 1
+                continue
             if needs_vae(batch, latent_source):
                 from .utils.dataset import frames_to_latents
                 latents = frames_to_latents(batch, vae, dev)        # raw clip -> resize/normalise kernel -> batched VAE encode
@@ -469,15 +508,36 @@ def main(
                     validation_sample(unet, vae, text_encoder, tokenizer, validation_data, os.path.join(output_dir, "samples"), global_step,
                                       batch.get("text_prompt", [""])[0] if isinstance(batch.get("text_prompt"), (list, tuple)) else "",
                                       dev, alphas_cumprod=abar, prediction_type=prediction_type)
+            if save_training_state and global_step % checkpointing_steps == 0:
+                save_state(os.path.join(output_dir, f"checkpoint-{global_step}"))
             if global_step >= max_train_steps:
                 break
+        skip_batches = 0   # the reference skips in the first epoch only
+    if resume_rng is not None:   # resumed at or past max_train_steps: no epoch ran
+        TS.restore_rng(resume_rng, dev)
     if world > 1:
         dist.barrier()
     if rank == 0:
         save_checkpoint(unet, lora_manager, output_dir, global_step, use_unet_lora, save_pretrained_model, final=True,
                         pretrained_model_path=pretrained_model_path, ema=optimizer if use_ema else None,
                         text_encoder=text_encoder if use_text_lora else None)
+    if save_training_state:
+        save_state(output_dir)
     return {"steps": global_step, "step_times": step_times, "stepper": stepper, "optimizer": optimizer}
+
+
+def _resume_target(resume_from_checkpoint, output_dir):
+    """The checkpoint folder to resume from: a `checkpoint-N/` folder or a final `output_dir`; "latest" / True: the one under
+    output_dir with the complete training state of the highest step (None, a fresh start, when there is none yet)."""
+    if resume_from_checkpoint is None or resume_from_checkpoint is False or resume_from_checkpoint == "":
+        return None
+    if resume_from_checkpoint is True or resume_from_checkpoint == "latest":
+        from .training_state import latest
+        found = latest(output_dir)
+        if found is None:
+            print(f"resume_from_checkpoint={resume_from_checkpoint!r}: no complete training state under {output_dir}; starting from step 0")
+        return found
+    return str(resume_from_checkpoint)
 
 
 @contextlib.contextmanager

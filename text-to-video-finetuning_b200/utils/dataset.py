@@ -404,6 +404,15 @@ class ShapeGroupedBatches:
         if self.single_key:
             self._agree(None)
 
+    def state_dict(self):
+        """The items waiting in the buffers (the items themselves: reading them again would draw new random frame windows)
+        and the single_key group key."""
+        return {"buffers": [(k, list(v)) for k, v in self.buffers.items()], "key": self._key}
+
+    def load_state_dict(self, state):
+        self.buffers = {tuple(k): list(v) for k, v in state["buffers"]}
+        self._key = None if state["key"] is None else tuple(state["key"])
+
     def _agree(self, error):
         """One all-reduce (MAX) of [error, key, -key], the key as 5 integers: the ranks' keys agree iff max == -max(-key)."""
         import torch.distributed as dist
@@ -418,6 +427,51 @@ class ShapeGroupedBatches:
                              "(frames, height, width) group: grouping different shapes across ranks is not supported. "
                              + (error or "another rank met a different group key") + ". Use one target size and one "
                              "n_sample_frames (no use_bucketing, no mix of images and videos), or train_batch_size 1.")
+
+
+class EpochOrder(torch.utils.data.Sampler):
+    """The item order of one epoch of `base` (a RandomSampler, SequentialSampler or DistributedSampler) and how many of its
+    items have been handed out, so a resumed run continues at the same item of the same shuffle.
+
+    A RandomSampler without a generator seeds itself with one int64 drawn from torch's default CPU generator when its pass
+    starts; that same draw is made here, recorded in `seed` and handed to the sampler as its generator, so the order and the
+    generator's stream are exactly those of the plain sampler.  A DistributedSampler's order is its (seed, epoch) and a
+    SequentialSampler's is fixed.  `resume(state)` makes the next pass replay the recorded shuffle (no draw) and skip the
+    items already consumed."""
+
+    def __init__(self, base):
+        self.base = base
+        self.draws = isinstance(base, torch.utils.data.RandomSampler) and base.generator is None
+        self.seed, self.consumed, self._resume = None, 0, None
+
+    def __len__(self):
+        return len(self.base)
+
+    def __iter__(self):
+        resume, self._resume = self._resume, None
+        if self.draws:
+            self.seed = resume["seed"] if resume else int(torch.empty((), dtype=torch.int64).random_().item())
+            self.base.generator = torch.Generator()
+            self.base.generator.manual_seed(self.seed)
+        self.consumed = 0
+        it = iter(self.base)
+        for _ in range(resume["consumed"] if resume else 0):
+            next(it)
+            self.consumed += 1
+        for i in it:
+            self.consumed += 1
+            yield i
+
+    def state_dict(self):
+        d = {"seed": self.seed, "consumed": self.consumed}
+        if isinstance(self.base, torch.utils.data.distributed.DistributedSampler):
+            d["sampler_seed"], d["sampler_epoch"] = self.base.seed, self.base.epoch
+        return d
+
+    def resume(self, state):
+        if "sampler_epoch" in state:
+            self.base.set_epoch(state["sampler_epoch"])
+        self._resume = dict(state)
 
 
 def _collate_group(items):
