@@ -236,6 +236,12 @@ int t2v_cast_f32_bf16(const float* src, void* dst, int64_t n, void* stream);
  * t2v_softmax_fwd's causal_period > 0 applies the encoder's causal mask (row r sees columns <= r % causal_period).         */
 int t2v_embed_tokens(const int64_t* ids, const float* tok_emb, const float* pos_emb, void* out, int64_t rows, int32_t L, int32_t C,
                      int32_t vocab, void* stream);
+/* Backward of t2v_embed_tokens for text-encoder training: dy bf16 [rows][C] (rows = B * L) is accumulated (+=) into the fp32
+ * gradients dtok [vocab][C] (dtok[id] += sum of the rows with that id, the id clamped to [0, vocab) as the forward clamps it)
+ * and dpos [>= L][C] (dpos[l] += sum over b of row b*L + l).  Either may be null (that table is frozen).  No atomics: each
+ * output row is summed by one block in row order, so two launches on the same inputs give the same bits.               */
+int t2v_embed_tokens_bwd(const int64_t* ids, const void* dy, float* dtok, float* dpos, int64_t rows, int32_t L, int32_t C,
+                         int32_t vocab, void* stream);
 int t2v_gelu_bf16(const void* x, void* y, int64_t n, int32_t quick, void* stream);
 /* Backward of t2v_gelu_bf16 for text-encoder LoRA training: dx = dy * gelu'(x), x the saved input, same `quick` switch;
  * n a multiple of 8.                                                                                                     */

@@ -198,6 +198,60 @@ __global__ void embed_tokens_kernel(const int64_t* __restrict__ ids, const float
         reinterpret_cast<uint4*>(out)[i] = pack8e(v);
     }
 }
+// Backward of embed_tokens_kernel, accumulated into the fp32 tables' gradients without atomics, so the sums are the same on
+// every launch.  Blocks [0, n_tok) are token blocks, one per row r: a block whose (clamped) id already occurs in an earlier row
+// exits, so exactly one block owns each id; it sums the rows with that id in row order and adds the sum to dtok[id] once.
+// Padded prompts repeat one id dozens of times, so most rows exit after the scan.  Blocks [n_tok, n_tok + n_pos) are
+// position blocks, one per l: dpos[l] += sum over b of dy[b*L + l], in b order.
+__global__ void embed_tokens_bwd_kernel(const int64_t* __restrict__ ids, const __nv_bfloat16* __restrict__ dy, float* __restrict__ dtok,
+                                        float* __restrict__ dpos, int64_t rows, int L, int C, int vocab, int n_tok) {
+    pdl_sync();
+    const int V = C >> 3;
+    auto clamp_id = [&](int64_t r) {
+        const int64_t id = __ldg(ids + r);
+        return id < 0 ? int64_t(0) : (id >= vocab ? int64_t(vocab - 1) : id);
+    };
+    if (int(blockIdx.x) < n_tok) {
+        const int64_t r = blockIdx.x;
+        const int64_t id = clamp_id(r);
+        int seen = 0;
+        for (int64_t j = threadIdx.x; j < r && !seen; j += blockDim.x) seen = clamp_id(j) == id;
+        if (__syncthreads_or(seen)) return;
+        for (int cv = threadIdx.x; cv < V; cv += blockDim.x) {
+            float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+            for (int64_t j = r; j < rows; ++j) {
+                if (clamp_id(j) != id) continue;
+                float v[8];
+                unpack8e(__ldg(reinterpret_cast<const uint4*>(dy + j * C) + cv), v);
+#pragma unroll
+                for (int k = 0; k < 8; ++k) acc[k] += v[k];
+            }
+            float4* g = reinterpret_cast<float4*>(dtok + id * C) + 2 * cv;
+            float4 a = g[0], b = g[1];
+            a.x += acc[0]; a.y += acc[1]; a.z += acc[2]; a.w += acc[3];
+            b.x += acc[4]; b.y += acc[5]; b.z += acc[6]; b.w += acc[7];
+            g[0] = a;
+            g[1] = b;
+        }
+        return;
+    }
+    const int l = int(blockIdx.x) - n_tok;
+    for (int cv = threadIdx.x; cv < V; cv += blockDim.x) {
+        float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+        for (int64_t j = l; j < rows; j += L) {
+            float v[8];
+            unpack8e(__ldg(reinterpret_cast<const uint4*>(dy + j * C) + cv), v);
+#pragma unroll
+            for (int k = 0; k < 8; ++k) acc[k] += v[k];
+        }
+        float4* g = reinterpret_cast<float4*>(dpos + int64_t(l) * C) + 2 * cv;
+        float4 a = g[0], b = g[1];
+        a.x += acc[0]; a.y += acc[1]; a.z += acc[2]; a.w += acc[3];
+        b.x += acc[4]; b.y += acc[5]; b.z += acc[6]; b.w += acc[7];
+        g[0] = a;
+        g[1] = b;
+    }
+}
 __global__ void geglu_bwd_kernel(const __nv_bfloat16* __restrict__ proj, const __nv_bfloat16* __restrict__ dout,
                                  __nv_bfloat16* __restrict__ dproj, int64_t M, int I) {
     pdl_sync();
@@ -703,6 +757,16 @@ int t2v_embed_tokens(const int64_t* ids, const float* tok_emb, const float* pos_
     if (C % 8) return fail(-2, "embed_tokens: C=%d must be a multiple of 8", C);
     launch_pdl(embed_tokens_kernel, dim3(ew_grid(rows * (C / 8))), dim3(256), size_t(0), ST, ids, tok_emb, pos_emb, BFW(out), rows, L, C, vocab);
     return launch_checked(int(cudaGetLastError()), "embed_tokens");
+}
+int t2v_embed_tokens_bwd(const int64_t* ids, const void* dy, float* dtok, float* dpos, int64_t rows, int32_t L, int32_t C, int32_t vocab,
+                         void* stream) {
+    if (C % 8) return fail(-2, "embed_tokens_bwd: C=%d must be a multiple of 8", C);
+    if (rows <= 0 || L <= 0 || rows % L || vocab <= 0) return fail(-2, "embed_tokens_bwd: rows=%lld, L=%d, vocab=%d", (long long)rows, L, vocab);
+    if (rows > INT32_MAX) return fail(-2, "embed_tokens_bwd: rows=%lld too large", (long long)rows);
+    const int n_tok = dtok ? int(rows) : 0, n_pos = dpos ? L : 0;
+    if (n_tok + n_pos == 0) return 0;
+    launch_pdl(embed_tokens_bwd_kernel, dim3(n_tok + n_pos), dim3(128), size_t(0), ST, ids, BF(dy), dtok, dpos, rows, L, C, vocab, n_tok);
+    return launch_checked(int(cudaGetLastError()), "embed_tokens_bwd");
 }
 int t2v_silu_f32_to_bf16(const float* x, void* y, int64_t n, int32_t apply_silu, void* stream) {
     launch_pdl(silu_f32_to_bf16_kernel, dim3(ew_grid(n)), dim3(256), size_t(0), ST, x, BFW(y), n, apply_silu);

@@ -445,6 +445,33 @@ def layer_norm(x, gamma, beta, eps=1e-5):
     return _LayerNorm.apply(x, gamma, beta, eps)
 
 
+# ---------------------------------------------------------------------------------------------------- embeddings
+class _EmbedTokens(Function):
+    """x [B*L, C] bf16 = tok[ids] + pos[l] from the fp32 tables; the backward accumulates the tables' gradients (the trainable
+    ones) with the deterministic embed_tokens_bwd kernel."""
+
+    @staticmethod
+    def forward(ctx, ids, tok, pos):
+        ctx.save_for_backward(ids)
+        ctx.tok, ctx.pos = tok, pos
+        return prims.embed_tokens(ids, _cont(_f32(tok)), _cont(_f32(pos)))
+
+    @staticmethod
+    def backward(ctx, dy):
+        ids, = ctx.saved_tensors
+        tok, pos = ctx.tok, ctx.pos
+        dtok = grad_vec(tok) if tok.requires_grad else None
+        dpos = grad_vec(pos) if pos.requires_grad else None
+        dy = _cont(dy)
+        _run_param_grads(lambda: prims.embed_tokens_bwd(ids, dy, dtok, dpos, tok.shape[0]), dy, ids)
+        return None, None, None
+
+
+def embed_tokens(ids, tok, pos):
+    """ids int64 [B, L] -> [B*L, C] bf16 (CLIPTextEmbeddings); differentiable in the token and position tables."""
+    return _EmbedTokens.apply(ids, tok, pos)
+
+
 # ---------------------------------------------------------------------------------------------------- activations
 class _Geglu(Function):
     @staticmethod

@@ -583,6 +583,20 @@ def embed_tokens(ids, tok_emb, pos_emb):
     return out
 
 
+def embed_tokens_bwd(ids, dy, dtok, dpos, vocab):
+    """Backward of embed_tokens, accumulated: dtok fp32 [vocab, C][id] += sum of the rows of dy bf16 [B*L, C] with that (clamped)
+    id, dpos fp32 [>= L, C][l] += sum over b of row (b, l).  Either gradient may be None (frozen table).  Deterministic."""
+    assert ids.dtype == torch.int64 and ids.is_cuda and ids.is_contiguous()
+    _chk_bf16(dy)
+    _chk_f32(dtok, dpos)
+    B, L = ids.shape
+    C = dy.shape[1]
+    assert dy.shape[0] == B * L, (dy.shape, ids.shape)
+    assert dtok is None or dtok.shape == (vocab, C), (dtok.shape, vocab, C)
+    assert dpos is None or (dpos.shape[0] >= L and dpos.shape[1] == C), (dpos.shape, L, C)
+    native.check(native.lib().t2v_embed_tokens_bwd(_p(ids), _p(dy), _p(dtok), _p(dpos), B * L, L, C, int(vocab), _stream()))
+
+
 def softmax_bwd(p, dp, n_valid, scale):
     _chk_bf16(p)
     _chk_f32(dp)

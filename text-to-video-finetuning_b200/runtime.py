@@ -20,10 +20,16 @@ def _align(n, a=64):
     return (n + a - 1) // a * a
 
 
+def _has_shadow(p):
+    """GEMM weights (rank >= 2) get a bf16 compute copy; a lookup table marked `_t2v_lookup` (an embedding, gathered from its
+    fp32 master) is stored with the vectors instead, so no shadow is kept or rewritten for it."""
+    return p.dim() >= 2 and not getattr(p, "_t2v_lookup", False)
+
+
 class ParamArena:
     """Adopts a module's parameters into flat buffers.  Parameters keep their identity, shape, strides and names;
-    only their storage moves.  `param.grad` becomes a view into the flat gradient buffer and matrix-like weights get a
-    `_t2v_shadow` bf16 view in kernel layout ([Cout, KH, KW, Cin] / [out, 1, 1, in])."""
+    only their storage moves.  `param.grad` becomes a view into the flat gradient buffer and matrix-like weights (not
+    lookup tables) get a `_t2v_shadow` bf16 view in kernel layout ([Cout, KH, KW, Cin] / [out, 1, 1, in])."""
 
     def __init__(self, module, device=None, extra=()):
         # extra: parameters outside `module` to adopt as well (the text-encoder LoRA factors of a text-LoRA run)
@@ -38,8 +44,8 @@ class ParamArena:
         # matrices first (they need a bf16 shadow), then vectors; inside each class the TRAINABLE parameters come first (in
         # registration order), so the gradients that have to cross NVLink form two compact spans - 29 M elements instead of
         # 1.44 B for a LoRA run - and a block's trainable matrices stay one contiguous range.
-        mats = [p for p in params if p.dim() >= 2]
-        vecs = [p for p in params if p.dim() < 2]
+        mats = [p for p in params if _has_shadow(p)]
+        vecs = [p for p in params if not _has_shadow(p)]
         mats = [p for p in mats if p.requires_grad] + [p for p in mats if not p.requires_grad]
         vecs = [p for p in vecs if p.requires_grad] + [p for p in vecs if not p.requires_grad]
         self.params = mats + vecs
@@ -60,7 +66,7 @@ class ParamArena:
             for p, o in zip(self.params, offs):
                 n = p.numel()
                 src = p.detach().to(device)
-                phys = ops._phys(src) if p.dim() >= 2 else src
+                phys = ops._phys(src) if _has_shadow(p) else src
                 if not phys.is_contiguous():
                     raise ValueError("conv weights must be in channels_last memory format before adoption")
                 self.master[o:o + n].copy_(phys.reshape(-1))
@@ -68,7 +74,7 @@ class ParamArena:
                 p.data = view
                 # frozen parameters keep grad None, so optimizers skip them exactly as they do in the reference
                 p.grad = torch.as_strided(self.grad, p.shape, p.stride(), o) if p.requires_grad else None
-                if p.dim() >= 2:
+                if _has_shadow(p):
                     p._t2v_shadow = self.shadow[o:o + n].view(ops._phys(view).shape)
         self.offsets = offs
         self._attach_fused(module, {id(p): o for p, o in zip(self.params, offs)})

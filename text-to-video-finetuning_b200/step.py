@@ -123,12 +123,15 @@ class DataParallelStep:
 
     `prediction_type` picks the loss target of every pass: the noise ('epsilon') or the velocity ('v_prediction').
 
-    `text_encoder` (a text_encoder.CLIPTextModel with cloneofsimo LoRA injected, `use_text_lora`): the call then takes the
-    prompt token ids (B, L) in place of the text states, and the step follows train.py:803-834: the encoder runs once, in
-    the step (and the graph); with passes=2 and F > 1, pass 0 is the full clip on the detached states and pass 1 only frame
-    1 of the clip on the trainable states - the one pass whose gradient reaches the text LoRA; with F = 1 one pass on the
-    trainable states.  The arena adopts the LoRA factors next to the UNet's parameters (never the frozen encoder weights),
-    so clipping, the optimizers and the EMA cover them."""
+    `text_encoder` (a text_encoder.CLIPTextModel that trains: cloneofsimo LoRA injected, `use_text_lora`, and/or parameters
+    unfrozen by `train_text_encoder`): the call then takes the prompt token ids (B, L) in place of the text states, and the
+    step follows train.py:803-834: the encoder runs once, in the step (and the graph); with passes=2 and F > 1, pass 0 is the
+    full clip on the detached states and pass 1 only frame 1 of the clip on the trainable states - the one pass whose
+    gradient reaches the text encoder; with F = 1 one pass on the trainable states.  The arena adopts the trainable text
+    tensors next to the UNet's parameters, so clipping, the optimizers and the EMA cover them.  With LoRA only, those are the
+    LoRA factors (the frozen encoder weights stay outside); when base weights train, every text parameter is adopted, as the
+    UNet's are, so the text optimizer group (which lists the frozen ones too, train.py:579-595) lives in the arena and the
+    trainable projection weights are read through the arena's bf16 shadow."""
 
     def __init__(self, unet, alphas_cumprod, passes=1, use_graph=False, adopt=True, optimizer=None, accumulation=1,
                  prediction_type="epsilon", text_encoder=None):
@@ -139,7 +142,10 @@ class DataParallelStep:
         self.prediction_type = prediction_type
         self.passes = passes
         self.text_encoder = text_encoder
-        text_params = [p for p in text_encoder.parameters() if p.requires_grad] if text_encoder is not None else ()
+        text_params = ()
+        if text_encoder is not None:
+            every = text_encoder.base_trains()
+            text_params = [p for p in text_encoder.parameters() if p.requires_grad or every]
         self.arena = ParamArena(unet, extra=text_params) if adopt else None
         self.use_graph = use_graph
         self.sync_gradients = True   # set False to run fwd+bwd only (profiling on a single rank)

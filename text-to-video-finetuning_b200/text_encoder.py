@@ -11,9 +11,13 @@ launch-bound, not worth a fused kernel) -> output projection with the residual i
 GELU -> fc2 (+ residual epilogue).  Embedding lookup (token + position) is one kernel; final LayerNorm as in
 CLIPTextTransformer.
 
-Encoder with cloneofsimo LoRA wrappers (`use_text_lora`, train.py:571-572): `encode` runs the same layers as autograd ops
-(ops.py), each projection through its wrapper (utils/lora.lora_linear_forward), so the LoRA factors get gradients and the
-eval forward applies them.  The frozen base weights are cast to bf16 once (`_t2v_shadow`); no embedding gradient is formed."""
+Encoder that trains (cloneofsimo LoRA wrappers, `use_text_lora`, train.py:571-572; and/or unfrozen parameters,
+`train_text_encoder` with `trainable_text_modules`, train.py:579-595): `encode` runs the same layers as autograd ops (ops.py),
+each projection through its wrapper (utils/lora.lora_linear_forward) or as a plain linear, so every trainable tensor - LoRA
+factors, projection weights and biases, LayerNorm affines, token and position embeddings - gets its gradient, and the eval
+forward (`forward`, then `encode` without a tape) reads the current weights.  A trainable projection weight is read through
+its parameter-arena shadow (ops.weight_bf16), which the fused optimizer rewrites every step; a frozen one is cast to bf16
+once (`_t2v_shadow`).  Embeddings: with LoRA only, no embedding gradient is formed (the tables are frozen)."""
 import json
 import os
 from types import SimpleNamespace
@@ -51,6 +55,8 @@ class CLIPTextEmbeddings(nn.Module):
         super().__init__()
         self.token_embedding = nn.Embedding(vocab, C)
         self.position_embedding = nn.Embedding(positions, C)
+        for e in (self.token_embedding, self.position_embedding):
+            e.weight._t2v_lookup = True   # gathered in fp32 by embed_tokens: the parameter arena keeps no bf16 copy of it
 
 
 class CLIPEncoder(nn.Module):
@@ -133,10 +139,19 @@ class CLIPTextModel(nn.Module):
         from .utils.lora import _WRAPPERS
         return any(isinstance(m, _WRAPPERS) for m in self.modules())
 
+    def trains(self):
+        """True when LoRA is injected or any parameter trains: the weights may then change, and `forward` runs `encode`."""
+        return self.lora_injected() or any(p.requires_grad for p in self.parameters())
+
+    def base_trains(self):
+        """True when a parameter of the encoder itself (not a LoRA factor) trains (`train_text_encoder`)."""
+        return any(p.requires_grad for n, p in self.named_parameters() if "lora" not in n)
+
     def forward(self, input_ids, attention_mask=None, **unused):
         """input_ids (B, L) int64 -> (last_hidden_state (B, L, hidden) fp32,).  The causal mask is always applied and, like
-        the reference's call (train.py:786), no padding mask is.  With LoRA injected this is `encode` (differentiable)."""
-        if self.lora_injected():
+        the reference's call (train.py:786), no padding mask is.  An encoder that trains runs `encode` (differentiable, and
+        reading the current weights); a frozen one the no-grad forward over bf16 weights packed once."""
+        if self.trains():
             B, L = input_ids.shape
             return (self.encode(input_ids).float().view(B, L, -1),)
         return self._forward_frozen(input_ids)
@@ -152,8 +167,8 @@ class CLIPTextModel(nn.Module):
                 w._t2v_shadow = prims.cast_f32_bf16(w.detach().float().contiguous()).view(w.shape[0], 1, 1, w.shape[1])
 
     def encode(self, input_ids):
-        """Autograd forward of an encoder with LoRA wrappers: input_ids (B, L) -> bf16 token matrix [B*L, hidden], the
-        final-LayerNorm output.  Gradients reach the LoRA factors only (base weights, norms and embeddings are frozen)."""
+        """Autograd forward: input_ids (B, L) -> bf16 token matrix [B*L, hidden], the final-LayerNorm output.  Gradients reach
+        every tensor with requires_grad (LoRA factors, and with train_text_encoder the unfrozen weights, norms and embeddings)."""
         from .layers import run_linear
         cfg = self.config
         ids = input_ids.to(torch.int64).contiguous()
@@ -162,8 +177,7 @@ class CLIPTextModel(nn.Module):
         quick = cfg.hidden_act == "quick_gelu"
         emb = self.text_model.embeddings
         self._frozen_shadows()
-        x = prims.embed_tokens(ids, emb.token_embedding.weight.detach().float().contiguous(),
-                               emb.position_embedding.weight.detach().float().contiguous())          # [B*L, C] bf16
+        x = ops.embed_tokens(ids, emb.token_embedding.weight, emb.position_embedding.weight)          # [B*L, C] bf16
         for lyr in self.text_model.encoder.layers:
             a, ln1, ln2 = lyr.self_attn, lyr.layer_norm1, lyr.layer_norm2
             res, h = ops.fork(x)

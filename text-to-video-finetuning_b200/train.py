@@ -15,7 +15,8 @@ classes (utils/dataset.py: OpenCV decode -> ONE resize + normalise kernel on the
 (utils.dataset.ShapeGroupedBatches; batch size 1 keeps the plain DataLoader); with data parallelism every rank must then see
 a single group.  Prompts go through the frozen CLIP text encoder (text_encoder.py) with a
 per-prompt embedding cache; a batch that already carries `text_embeds` skips it.  `use_text_lora` (cloneofsimo only) injects
-LoRA into the text encoder (train.py:571-572) and runs it inside the step on every batch's `prompt_ids` (step.py).
+LoRA into the text encoder (train.py:571-572), `train_text_encoder` with `trainable_text_modules` unfreezes its parameters by
+name (train.py:579-595, 763-773); either way the encoder runs inside the step on every batch's `prompt_ids` (step.py).
 Checkpoints (8(f) row 4): LoRA in the cloneofsimo list format or the stable_lora safetensors files (full weights and the webui
 file), the UNet in diffusers layout, and - when the pretrained folder
 is a full pipeline - the complete pipeline directory (`save_pipe`, train.py:395-449), plus a validation sample every
@@ -260,9 +261,10 @@ def main(
     if world > 1 and not dist.is_initialized():
         os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
         dist.init_process_group("nccl", device_id=dev)
-    if train_text_encoder:
-        raise NotImplementedError("train_text_encoder (full text-encoder training) is not implemented; use_text_lora with "
-                                  "lora_version 'cloneofsimo' trains a LoRA of the text encoder")
+    if train_text_encoder and trainable_text_modules is None:
+        # the reference trains no text parameter then (the encoder stays frozen, train.py:543, 579): refuse, do not train nothing
+        raise NotImplementedError("train_text_encoder needs trainable_text_modules (e.g. ['all']) to name the text-encoder "
+                                  "parameters to train; use_text_lora with lora_version 'cloneofsimo' trains a LoRA of it")
     if use_text_lora and lora_version == "stable_lora":
         raise NotImplementedError("use_text_lora is implemented for lora_version 'cloneofsimo' only")
     # text_encoder_gradient_checkpointing is accepted and has no effect: the text activations are 77 tokens per prompt
@@ -301,14 +303,21 @@ def main(
                                text_encoder_replace_modules=list(text_encoder_lora_modules), lora_bias=lora_bias)
     unet_lora_params, unet_negation = lora_manager.add_lora_to_model(use_unet_lora, unet, lora_manager.unet_replace_modules,
                                                                      lora_unet_dropout, lora_path, r=lora_rank)
-    text_encoder = text_lora_params = None
-    if use_text_lora:   # the text encoder and its LoRA must exist before the parameter arena is built
+    text_encoder = text_lora_params = text_negation = None
+    text_trains = use_text_lora or train_text_encoder
+    if text_trains:   # the text encoder, its LoRA and its trainable set must exist before the parameter arena is built
         from .text_encoder import CLIPTextModel
+        switch = "use_text_lora" if use_text_lora else "train_text_encoder"
         text_encoder = _load_optional(CLIPTextModel, pretrained_model_path, "text_encoder")
         if text_encoder is None:
-            raise FileNotFoundError(f"use_text_lora needs the text encoder of the pipeline: {pretrained_model_path}/text_encoder is missing")
-        text_lora_params, _ = lora_manager.add_lora_to_model(True, text_encoder, lora_manager.text_encoder_replace_modules,
-                                                             lora_text_dropout, lora_path, r=lora_rank)
+            raise FileNotFoundError(f"{switch} needs the text encoder of the pipeline: {pretrained_model_path}/text_encoder is missing")
+        text_lora_params, text_negation = lora_manager.add_lora_to_model(use_text_lora, text_encoder,
+                                                                         lora_manager.text_encoder_replace_modules,
+                                                                         lora_text_dropout, lora_path, r=lora_rank)
+        if train_text_encoder:   # train.py:768-773 (the reference applies it on the first step, before any update)
+            handle_trainable_modules(text_encoder, trainable_text_modules, is_enabled=True, negation=text_negation)
+            if not text_encoder.base_trains():
+                raise ValueError(f"trainable_text_modules={list(trainable_text_modules)!r} matches no text-encoder parameter")
         text_encoder = text_encoder.to(dev).train()
     unet = unet.to(dev)
     unet.train()
@@ -320,10 +329,11 @@ def main(
     unet._set_gradient_checkpointing(gradient_checkpointing)
 
     extra_unet_params = extra_unet_params or {}
-    # train.py:581-595: UNet, text encoder (train_text_encoder only, refused above), text LoRA, UNet LoRA; the text LoRA group
-    # takes extra_unet_params, as in the reference (SURVEY H4)
+    # train.py:581-595: UNet, text encoder (train_text_encoder), text LoRA, UNet LoRA; the text-encoder and text LoRA groups
+    # take extra_unet_params, as in the reference (SURVEY H4)
     groups = create_optimizer_params([
         param_optim(unet, trainable_modules is not None, extra_params=extra_unet_params, negation=unet_negation),
+        param_optim(text_encoder, train_text_encoder, extra_params=extra_unet_params, negation=text_negation),
         param_optim(text_lora_params, use_text_lora, is_lora=True, extra_params={**{"lr": learning_rate}, **extra_unet_params}),
         param_optim(unet_lora_params, use_unet_lora, is_lora=True, extra_params={**{"lr": learning_rate}, **extra_unet_params}),
     ], learning_rate)
@@ -368,7 +378,7 @@ def main(
             from transformers import CLIPTokenizer
             tokenizer = CLIPTokenizer.from_pretrained(pretrained_model_path, subfolder="tokenizer")
     # a text encoder that trains is run by the step on every batch: no embedding cache
-    embed_text = TextEmbedder(text_encoder, dev) if text_encoder is not None and not use_text_lora else None
+    embed_text = TextEmbedder(text_encoder, dev) if text_encoder is not None and not text_trains else None
     if cached_latent_dir:
         dataset = CachedLatents(cached_latent_dir)
     elif "synthetic" in kinds:
@@ -461,9 +471,9 @@ def main(
                 latents = frames_to_latents(batch, vae, dev)        # raw clip -> resize/normalise kernel -> batched VAE encode
             else:
                 latents = batch["pixel_values"].to(dev, torch.float32)
-            if use_text_lora:   # the step encodes the token ids itself
+            if text_trains:   # the step encodes the token ids itself
                 if "prompt_ids" not in batch:
-                    raise ValueError("use_text_lora trains the text encoder, so every batch needs 'prompt_ids'; this one has "
+                    raise ValueError(f"{switch} trains the text encoder, so every batch needs 'prompt_ids'; this one has "
                                      f"{sorted(batch)} (the synthetic dataset and a latent cache of text_embeds only have none)")
                 text = batch["prompt_ids"].reshape(latents.shape[0], -1).to(dev, torch.int64)
             elif "text_embeds" in batch:
@@ -499,12 +509,12 @@ def main(
             if rank == 0 and global_step % checkpointing_steps == 0:
                 save_checkpoint(unet, lora_manager, output_dir, global_step, use_unet_lora, save_pretrained_model,
                                 pretrained_model_path=pretrained_model_path, ema=optimizer if use_ema else None,
-                                text_encoder=text_encoder if use_text_lora else None)
+                                text_encoder=text_encoder if text_trains else None)
             if rank == 0 and validation_data and validation_steps and global_step % validation_steps == 0 and vae is not None \
                     and text_encoder is not None and tokenizer is not None and getattr(vae, "decoder", None) is not None:
                 from .sampling import validation_sample
                 with optimizer.ema_weights() if use_ema else contextlib.nullcontext(), \
-                        _text_preview(text_encoder) if use_text_lora else contextlib.nullcontext():   # preview what a user would export
+                        _text_preview(text_encoder) if text_trains else contextlib.nullcontext():   # preview what a user would export
                     validation_sample(unet, vae, text_encoder, tokenizer, validation_data, os.path.join(output_dir, "samples"), global_step,
                                       batch.get("text_prompt", [""])[0] if isinstance(batch.get("text_prompt"), (list, tuple)) else "",
                                       dev, alphas_cumprod=abar, prediction_type=prediction_type)
@@ -520,7 +530,7 @@ def main(
     if rank == 0:
         save_checkpoint(unet, lora_manager, output_dir, global_step, use_unet_lora, save_pretrained_model, final=True,
                         pretrained_model_path=pretrained_model_path, ema=optimizer if use_ema else None,
-                        text_encoder=text_encoder if use_text_lora else None)
+                        text_encoder=text_encoder if text_trains else None)
     if save_training_state:
         save_state(output_dir)
     return {"steps": global_step, "step_times": step_times, "stepper": stepper, "optimizer": optimizer}
@@ -542,7 +552,7 @@ def _resume_target(resume_from_checkpoint, output_dir):
 
 @contextlib.contextmanager
 def _text_preview(text_encoder):
-    """The validation preview encodes through the LoRA text encoder in eval mode (LoRA dropout off) and without a tape."""
+    """The validation preview encodes through the trained text encoder in eval mode (LoRA dropout off) and without a tape."""
     was = text_encoder.training
     text_encoder.eval()
     try:
@@ -591,16 +601,18 @@ def save_checkpoint(unet, lora_manager, output_dir, step, use_unet_lora, save_pr
         strict=True (the reference writes the lora_A / lora_B keys into unet/ as well, which a plain UNet load rejects).
     ema (`use_ema`): the optimizer holding the EMA of the weights; the EMA weights are then written as well: the LoRA files
     with an `_ema` suffix and (save_pretrained_model) `unet_ema/` in the diffusers UNet layout.
-    text_encoder (`use_text_lora`): `lora/<step>_text_encoder.pt` (and `_ema`) in the same list format, and with
-    save_pretrained_model `text_encoder/model.safetensors` holding the LoRA collapsed into the plain Hugging Face keys (the
-    reference writes the wrapper keys, which transformers.CLIPTextModel does not load as the trained encoder)."""
+    text_encoder (`use_text_lora` / `train_text_encoder`): with LoRA injected, `lora/<step>_text_encoder.pt` (and `_ema`) in
+    the same list format; with save_pretrained_model `text_encoder/model.safetensors` holding the trained encoder under the
+    plain Hugging Face keys, any LoRA collapsed into its base weight (the reference writes the wrapper keys, which
+    transformers.CLIPTextModel does not load as the trained encoder).  When the encoder's own weights train and ema is given,
+    `text_encoder_ema/` holds the EMA weights in the same layout."""
     path = output_dir if final else os.path.join(output_dir, f"checkpoint-{step}")
     os.makedirs(path, exist_ok=True)
     stable = use_unet_lora and lora_manager.is_stable_lora()
     lora_dir = os.path.join(path, "lora")
 
     def save_lora(suffix=""):
-        if text_encoder is not None:
+        if text_encoder is not None and text_encoder.lora_injected():
             from .utils.lora import save_lora_weight
             os.makedirs(lora_dir, exist_ok=True)
             save_lora_weight(text_encoder, os.path.join(lora_dir, f"{step}_text_encoder{suffix}.pt"), lora_manager.text_encoder_replace_modules)
@@ -626,16 +638,27 @@ def save_checkpoint(unet, lora_manager, output_dir, step, use_unet_lora, save_pr
         else:
             unet.save_pretrained(os.path.join(path, "unet"), state_dict=unet_sd())
         if text_encoder is not None and os.path.isdir(os.path.join(path, "text_encoder")):
-            from safetensors.torch import save_file
-            te_dir = os.path.join(path, "text_encoder")
-            if os.path.isfile(os.path.join(te_dir, "pytorch_model.bin")):   # the pretrained weights copied by save_pipe
-                os.remove(os.path.join(te_dir, "pytorch_model.bin"))
-            save_file(text_encoder.plain_state_dict(), os.path.join(te_dir, "model.safetensors"), metadata={"format": "pt"})
+            save_text_encoder(text_encoder, os.path.join(path, "text_encoder"))
     if ema is not None:
         with ema.ema_weights():
             save_lora("_ema")
             if save_pretrained_model:
                 unet.save_pretrained(os.path.join(path, "unet_ema"), state_dict=unet_sd())
+                if text_encoder is not None and text_encoder.base_trains() and os.path.isdir(os.path.join(path, "text_encoder")):
+                    import shutil
+                    ema_dir = os.path.join(path, "text_encoder_ema")
+                    os.makedirs(ema_dir, exist_ok=True)
+                    shutil.copyfile(os.path.join(path, "text_encoder", "config.json"), os.path.join(ema_dir, "config.json"))
+                    save_text_encoder(text_encoder, ema_dir)
+
+
+def save_text_encoder(text_encoder, te_dir):
+    """The encoder's current weights as `te_dir/model.safetensors` under the plain Hugging Face keys (next to the config.json
+    save_pipe copied); a pretrained `pytorch_model.bin` there is removed, so the folder holds one set of weights."""
+    from safetensors.torch import save_file
+    if os.path.isfile(os.path.join(te_dir, "pytorch_model.bin")):
+        os.remove(os.path.join(te_dir, "pytorch_model.bin"))
+    save_file(text_encoder.plain_state_dict(), os.path.join(te_dir, "model.safetensors"), metadata={"format": "pt"})
 
 
 def load_config(path):
