@@ -179,9 +179,11 @@ def _gemm_allocators(prims):
             "dropout_scale_add": dropout_scale_add, "gelu_bwd": gelu_bwd}
 
 
-def _unet_step(B, F, hw, lora=False):
+def _unet_step(B, F, hw, lora=False, prediction_type="epsilon", text=None):
     """One training pass of the full-size UNet over the step's parameter arena (fused projections), as DataParallelStep
-    runs it; `lora`: the bench's cloneofsimo rank-16 LoRA on every UNet linear (q / k / v then stay separate GEMMs)."""
+    runs it; `lora`: the bench's cloneofsimo rank-16 LoRA on every UNet linear (q / k / v then stay separate GEMMs);
+    `prediction_type`: the loss target (the velocity loss of a v-prediction step); `text`: the text states (B, 77, 1024), by
+    default frozen zeros (a trained text encoder hands states that need a gradient)."""
     import torch
 
     from t2v_b200 import step as S
@@ -203,8 +205,9 @@ def _unet_step(B, F, hw, lora=False):
             mod.p = 0.0
     ParamArena(m, device=dev)
     lat, noise = torch.zeros(B, 4, F, *hw, device=dev), torch.zeros(B, 4, F, *hw, device=dev)
-    ehs = torch.zeros(B, 77, 1024, device=dev)
-    loss = S.finetune_loss(m, lat, noise, torch.full((B,), 417, device=dev), ehs, L.ddpm_alphas_cumprod().to(dev))
+    ehs = torch.zeros(B, 77, 1024, device=dev) if text is None else text
+    loss = S.finetune_loss(m, lat, noise, torch.full((B,), 417, device=dev), ehs, L.ddpm_alphas_cumprod().to(dev),
+                           prediction_type=prediction_type)
     loss.backward()
 
 
