@@ -212,6 +212,29 @@ int t2v_mse_loss(const void* pred, const float* target, float* loss, const float
  * never stored.  abar (fp32 [T]) and timesteps (int64 [B]) are read on the device.  loss / gout / dpred as t2v_mse_loss. */
 int t2v_velocity_mse_loss(const void* pred, const float* x0, const float* noise, const float* alphas_cumprod, const int64_t* timesteps,
                           float* loss, const float* gout, void* dpred, int32_t B, int32_t C, int32_t F, int32_t HW, void* stream);
+/* Weighted and robust diffusion objectives (diffusers' --snr_gamma, --loss_type, --huber_schedule, --huber_c).  Per sample b,
+ * with a_b = abar[t_b], target y (noise, or the velocity above when prediction is T2V_PRED_V) and d = pred - y:
+ *   psi(d)  T2V_LOSS_L2: d^2   T2V_LOSS_HUBER: 2c_b (sqrt(d^2 + c_b^2) - c_b)   T2V_LOSS_SMOOTH_L1: 2 (sqrt(d^2 + c_b^2) - c_b)
+ *   c_b     T2V_HUBER_CONSTANT: huber_c   T2V_HUBER_EXPONENTIAL: huber_c^(t_b / T)
+ *           T2V_HUBER_SNR: (1 - huber_c) / (1 + sigma_b)^2 + huber_c, sigma_b = sqrt((1 - a_b) / a_b)   (huber_c at a_b = 0)
+ *   w_b     snr_gamma <= 0: 1.  Otherwise, snr_b = a_b / (1 - a_b): min(snr_b, gamma) / snr_b for T2V_PRED_EPSILON (1 at
+ *           a_b = 0), min(snr_b, gamma) / (snr_b + 1) for T2V_PRED_V (0 at a_b = 0)  (Hang et al. 2023, Min-SNR-gamma).
+ * loss != NULL: *loss = sum_e w_b(e) psi(d_e) / numel.  dpred != NULL: dpred = *gout * w_b psi'(d) / numel.  With
+ * T2V_LOSS_L2 and snr_gamma <= 0 this is t2v_mse_loss / t2v_velocity_mse_loss.  x0 is read only for T2V_PRED_V.        */
+enum { T2V_PRED_EPSILON = 0, T2V_PRED_V = 1 };
+enum { T2V_LOSS_L2 = 0, T2V_LOSS_HUBER = 1, T2V_LOSS_SMOOTH_L1 = 2 };
+enum { T2V_HUBER_CONSTANT = 0, T2V_HUBER_EXPONENTIAL = 1, T2V_HUBER_SNR = 2 };
+typedef struct {
+    int32_t prediction;      /* T2V_PRED_*                                                   */
+    int32_t loss;            /* T2V_LOSS_*                                                   */
+    int32_t huber_schedule;  /* T2V_HUBER_*, ignored under T2V_LOSS_L2                       */
+    int32_t num_timesteps;   /* T, the length of alphas_cumprod                              */
+    float huber_c;           /* > 0; <= 1 with T2V_HUBER_EXPONENTIAL                          */
+    float snr_gamma;         /* > 0: Min-SNR-gamma weighting; <= 0: none                      */
+} T2VLossParams;
+int t2v_diffusion_loss(const void* pred, const float* noise, const float* x0, const float* alphas_cumprod, const int64_t* timesteps,
+                       const T2VLossParams* params, float* loss, const float* gout, void* dpred, int32_t B, int32_t C, int32_t F,
+                       int32_t HW, void* stream);
 
 /* AutoencoderKL latent_dist.sample() + rearrange + * scale (train.py:343-345): moments [B*F][HW][8] bf16 (mean | logvar),
  * eps (B,4,F,HW) fp32 -> out (B,4,F,HW) fp32 = (mean + exp(0.5 clamp(logvar,-30,20)) eps) * scale.                    */

@@ -5,6 +5,7 @@
 #include "ptx.cuh"
 
 #include <algorithm>
+#include <cmath>
 #include <cuda_bf16.h>
 
 namespace t2v {
@@ -81,9 +82,53 @@ __global__ void from_nhwc8_kernel(const __nv_bfloat16* __restrict__ in, float* _
 // train.py:796-797).  abar and t are read on the device, so a replayed CUDA graph uses each step's timesteps.
 // Six blocks per SM holds the kernel at the 40 registers the noise-target-only version used (no spills); left free, ptxas
 // keeps all sixteen loads of the velocity path in flight and takes 42, which drops a block per SM for both objectives.
+//
+// The same body computes the weighted and robust objectives of t2v_diffusion_loss: FORM picks the per-element loss psi and
+// WEIGHTED the Min-SNR-gamma sample weight w_b; loss += sum w_b psi(e) / numel, dpred = g w_b psi'(e) / numel.  w_b and the
+// Huber scale c_b come from abar[t[b]] on the device, like the velocity, so a replayed graph uses each step's timesteps.
+// mse_kernel<kL2, false> is the plain MSE above: its body is unchanged, and `terms` is never read.
+enum LossForm { kL2 = 0, kHuber = 1, kSmoothL1 = 2 };   // = T2V_LOSS_*
+struct LossTerms {
+    float huber_c;      // c of T2V_HUBER_CONSTANT, and the floor of T2V_HUBER_SNR
+    float log_c_per_t;  // ln(huber_c) / T: T2V_HUBER_EXPONENTIAL's c_b = exp(t_b ln(huber_c) / T)
+    float snr_gamma;
+    int schedule;       // T2V_HUBER_*
+};
+
+// Min-SNR-gamma weight, snr = a / (1 - a), written without dividing by 1 - a:
+//   epsilon  min(snr, gamma) / snr       = min(1, gamma (1 - a) / a), whose limit at a = 0 (snr = 0) is 1;
+//   v        min(snr, gamma) / (snr + 1) = min(a, gamma (1 - a)), which is 0 at a = 0 without a special case.
+__device__ __forceinline__ float min_snr_weight(float a, float gamma, bool velocity) {
+    if (velocity) return fminf(a, gamma * (1.f - a));
+    return a > 0.f ? fminf(1.f, __fdividef(gamma * (1.f - a), a)) : 1.f;   // a in (0, 1]: both operands finite
+}
+// Huber scale of sample b.  T2V_HUBER_SNR: (1 - c) / (1 + sigma)^2 + c with sigma = sqrt((1 - a) / a) is
+// (1 - c) a / (sqrt(a) + sqrt(1 - a))^2 + c, whose denominator is >= 1: finite at a = 0, where it is c.
+__device__ __forceinline__ float huber_scale(const LossTerms& lt, float a, int64_t tb) {
+    if (lt.schedule == T2V_HUBER_EXPONENTIAL) return expf(float(tb) * lt.log_c_per_t);
+    if (lt.schedule == T2V_HUBER_SNR) {
+        const float s = sqrtf(a) + sqrtf(1.f - a);
+        return __fdividef((1.f - lt.huber_c) * a, s * s) + lt.huber_c;
+    }
+    return lt.huber_c;
+}
+// psi(e) and psi'(e) of the pseudo-Huber forms.  sqrt(e^2 + c^2) - c is formed as e^2 / (sqrt(e^2 + c^2) + c), which keeps
+// its relative precision for |e| << c.  c >= huber_c > 0, so both denominators are positive and finite.
+template <int FORM>
+__device__ __forceinline__ void huber_terms(float e, float c, float& psi, float& dpsi) {
+    const float q = fmaxf(fmaf(e, e, c * c), 1e-30f);   // c^2 underflows only for c < 1e-19
+    const float r = rsqrtf(q);                 // 1 / sqrt(e^2 + c^2)
+    const float k = FORM == kHuber ? 2.f * c : 2.f;
+    psi = __fdividef(k * e * e, fmaf(q, r, c));
+    dpsi = k * e * r;
+}
+
+template <int FORM, bool WEIGHTED>
 __global__ void __launch_bounds__(256, 6) mse_kernel(const __nv_bfloat16* __restrict__ pred, const float* __restrict__ target, float* __restrict__ loss,
                            const float* __restrict__ gout, __nv_bfloat16* __restrict__ dpred, int B, int C, int F, int HW,
-                           const float* __restrict__ x0, const float* __restrict__ abar, const int64_t* __restrict__ t) {
+                           const float* __restrict__ x0, const float* __restrict__ abar, const int64_t* __restrict__ t,
+                           LossTerms terms) {
+    constexpr bool kPlain = FORM == kL2 && !WEIGHTED;
     pdl_sync();
     const int64_t npix = int64_t(B) * F * HW;
     const float inv = 1.0f / (float(npix) * C);
@@ -94,13 +139,23 @@ __global__ void __launch_bounds__(256, 6) mse_kernel(const __nv_bfloat16* __rest
         const int f = int((i / HW) % F);
         const int b = int(i / (int64_t(HW) * F));
         const int64_t src = (int64_t(b) * C * F + f) * HW + hw, cstride = int64_t(F) * HW;
-        float sa = 1.f, sb = 0.f;
-        if (x0) {
-            const float a = abar[t[b]];
-            sa = sqrtf(a);
-            sb = sqrtf(1.f - a);
+        float sa = 1.f, sb = 0.f, a = 0.f, hc = 1.f;
+        if constexpr (kPlain) {
+            if (x0) {
+                const float a = abar[t[b]];
+                sa = sqrtf(a);
+                sb = sqrtf(1.f - a);
+            }
+        } else {
+            const int64_t tb = t[b];
+            a = abar[tb];
+            if (x0) {
+                sa = sqrtf(a);
+                sb = sqrtf(1.f - a);
+            }
+            if constexpr (FORM != kL2) hc = huber_scale(terms, a, tb);
         }
-        float v[8], d[8];
+        float v[8], d[8], px = 0.f;   // px: sum of psi over the pixel's channels, weighted once below
         unpack8e(__ldg(reinterpret_cast<const uint4*>(pred) + i), v);
 #pragma unroll
         for (int c = 0; c < 8; ++c) {
@@ -110,8 +165,23 @@ __global__ void __launch_bounds__(256, 6) mse_kernel(const __nv_bfloat16* __rest
                 if (x0) y = sa * y - sb * x0[src + c * cstride];
                 e = v[c] - y;
             }
-            acc += e * e;
-            d[c] = 2.f * e * inv * g;
+            if constexpr (kPlain) {
+                acc += e * e;
+                d[c] = 2.f * e * inv * g;
+            } else if constexpr (FORM == kL2) {
+                px += e * e;
+                d[c] = 2.f * e;
+            } else {
+                huber_terms<FORM>(e, hc, v[c], d[c]);   // v[c] <- psi, d[c] <- psi'
+                px += v[c];
+            }
+        }
+        if constexpr (!kPlain) {
+            const float w = WEIGHTED ? min_snr_weight(a, terms.snr_gamma, x0 != nullptr) : 1.f;
+            const float wg = w * inv * g;
+#pragma unroll
+            for (int c = 0; c < 8; ++c) d[c] *= wg;
+            acc = fmaf(w, px, acc);
         }
         if (dpred) reinterpret_cast<uint4*>(dpred)[i] = pack8e(d);
     }
@@ -699,8 +769,8 @@ int t2v_mse_loss(const void* pred, const float* target, float* loss, const float
                  int32_t F, int32_t HW, void* stream) {
     const int64_t n = int64_t(B) * F * HW;
     if (loss) cudaMemsetAsync(loss, 0, sizeof(float), ST);
-    launch_pdl(mse_kernel, dim3(ew_grid(n)), dim3(256), size_t(0), ST, BF(pred), target, loss, gout, BFW(dpred), B, C, F, HW,
-               (const float*)nullptr, (const float*)nullptr, (const int64_t*)nullptr);
+    launch_pdl(mse_kernel<kL2, false>, dim3(ew_grid(n)), dim3(256), size_t(0), ST, BF(pred), target, loss, gout, BFW(dpred), B, C, F,
+               HW, (const float*)nullptr, (const float*)nullptr, (const int64_t*)nullptr, LossTerms{});
     return launch_checked(int(cudaGetLastError()), "mse_loss");
 }
 int t2v_velocity_mse_loss(const void* pred, const float* x0, const float* noise, const float* alphas_cumprod, const int64_t* timesteps,
@@ -709,9 +779,41 @@ int t2v_velocity_mse_loss(const void* pred, const float* x0, const float* noise,
     if (C > 8) return fail(-2, "velocity_mse_loss: C=%d > 8", C);
     const int64_t n = int64_t(B) * F * HW;
     if (loss) cudaMemsetAsync(loss, 0, sizeof(float), ST);
-    launch_pdl(mse_kernel, dim3(ew_grid(n)), dim3(256), size_t(0), ST, BF(pred), noise, loss, gout, BFW(dpred), B, C, F, HW, x0,
-               alphas_cumprod, timesteps);
+    launch_pdl(mse_kernel<kL2, false>, dim3(ew_grid(n)), dim3(256), size_t(0), ST, BF(pred), noise, loss, gout, BFW(dpred), B, C, F,
+               HW, x0, alphas_cumprod, timesteps, LossTerms{});
     return launch_checked(int(cudaGetLastError()), "velocity_mse_loss");
+}
+int t2v_diffusion_loss(const void* pred, const float* noise, const float* x0, const float* alphas_cumprod, const int64_t* timesteps,
+                       const T2VLossParams* params, float* loss, const float* gout, void* dpred, int32_t B, int32_t C, int32_t F,
+                       int32_t HW, void* stream) {
+    if (!params) return fail(-2, "diffusion_loss: params is required");
+    const T2VLossParams& p = *params;
+    if (!noise || !alphas_cumprod || !timesteps) return fail(-2, "diffusion_loss: noise, alphas_cumprod and timesteps are required");
+    if (p.prediction != T2V_PRED_EPSILON && p.prediction != T2V_PRED_V) return fail(-2, "diffusion_loss: prediction %d", p.prediction);
+    if (p.prediction == T2V_PRED_V && !x0) return fail(-2, "diffusion_loss: v-prediction needs x0");
+    if (p.loss < T2V_LOSS_L2 || p.loss > T2V_LOSS_SMOOTH_L1) return fail(-2, "diffusion_loss: loss %d", p.loss);
+    if (p.loss != T2V_LOSS_L2) {
+        if (p.huber_schedule < T2V_HUBER_CONSTANT || p.huber_schedule > T2V_HUBER_SNR)
+            return fail(-2, "diffusion_loss: huber_schedule %d", p.huber_schedule);
+        if (!(p.huber_c > 0.f)) return fail(-2, "diffusion_loss: huber_c = %g must be > 0", double(p.huber_c));
+        if (p.huber_schedule == T2V_HUBER_EXPONENTIAL && (p.huber_c > 1.f || p.num_timesteps <= 0))
+            return fail(-2, "diffusion_loss: the exponential schedule needs 0 < huber_c <= 1 and T > 0");
+    }
+    if (C > 8) return fail(-2, "diffusion_loss: C=%d > 8", C);
+    const LossTerms lt{p.huber_c, p.num_timesteps > 0 ? float(std::log(double(p.huber_c)) / p.num_timesteps) : 0.f, p.snr_gamma,
+                       p.huber_schedule};
+    const float* v0 = p.prediction == T2V_PRED_V ? x0 : nullptr;   // the kernel forms the velocity when x0 is given
+    const bool weighted = p.snr_gamma > 0.f;
+    void (*kernel)(const __nv_bfloat16*, const float*, float*, const float*, __nv_bfloat16*, int, int, int, int, const float*,
+                   const float*, const int64_t*, LossTerms) =
+        p.loss == T2V_LOSS_HUBER     ? (weighted ? mse_kernel<kHuber, true> : mse_kernel<kHuber, false>)
+        : p.loss == T2V_LOSS_SMOOTH_L1 ? (weighted ? mse_kernel<kSmoothL1, true> : mse_kernel<kSmoothL1, false>)
+                                       : (weighted ? mse_kernel<kL2, true> : mse_kernel<kL2, false>);
+    const int64_t n = int64_t(B) * F * HW;
+    if (loss) cudaMemsetAsync(loss, 0, sizeof(float), ST);
+    launch_pdl(kernel, dim3(ew_grid(n)), dim3(256), size_t(0), ST, BF(pred), noise, loss, gout, BFW(dpred), B, C, F, HW, v0,
+               alphas_cumprod, timesteps, lt);
+    return launch_checked(int(cudaGetLastError()), "diffusion_loss");
 }
 int t2v_geglu_fwd(const void* proj, void* out, int64_t M, int32_t I, void* stream) {
     if (I % 8) return fail(-2, "geglu: inner dim %d not a multiple of 8", I);

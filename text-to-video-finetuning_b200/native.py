@@ -73,10 +73,16 @@ class GemmPlan(ctypes.Structure):
         ("st", ctypes.c_int32 * 5), ("follow", ctypes.c_int32)]
 
 
+class LossParams(ctypes.Structure):
+    """T2VLossParams: the objective of t2v_diffusion_loss (prediction, loss form, Huber schedule, huber_c, snr_gamma)."""
+    _fields_ = [("prediction", ctypes.c_int32), ("loss", ctypes.c_int32), ("huber_schedule", ctypes.c_int32),
+                ("num_timesteps", ctypes.c_int32), ("huber_c", ctypes.c_float), ("snr_gamma", ctypes.c_float)]
+
+
 EXPORTS = [
     "t2v_version", "t2v_last_error", "t2v_launch_count", "t2v_stream_capture_id", "t2v_channel_stats", "t2v_conv_fwd", "t2v_conv_dgrad", "t2v_conv_workspace_bytes", "t2v_conv_wgrad", "t2v_conv_wgrad_bias", "t2v_bgemm", "t2v_gemm_plan", "t2v_flash_attn_fwd", "t2v_flash_attn_bwd_splits", "t2v_flash_attn_bwd",
     "t2v_groupnorm_workspace_bytes", "t2v_groupnorm_fwd", "t2v_groupnorm_bwd", "t2v_layernorm_fwd", "t2v_layernorm_bwd",
-    "t2v_latents_to_nhwc8", "t2v_nhwc8_to_latents", "t2v_mse_loss", "t2v_velocity_mse_loss", "t2v_vae_sample", "t2v_geglu_fwd", "t2v_geglu_bwd", "t2v_silu_f32_to_bf16",
+    "t2v_latents_to_nhwc8", "t2v_nhwc8_to_latents", "t2v_mse_loss", "t2v_velocity_mse_loss", "t2v_diffusion_loss", "t2v_vae_sample", "t2v_geglu_fwd", "t2v_geglu_bwd", "t2v_silu_f32_to_bf16",
     "t2v_silu_bwd_f32", "t2v_silu_bf16", "t2v_silu_bf16_bwd", "t2v_add_bf16", "t2v_add_f32", "t2v_dropout_scale_add", "t2v_scale_bf16", "t2v_cast_f32_bf16", "t2v_embed_tokens", "t2v_embed_tokens_bwd", "t2v_gelu_bf16", "t2v_gelu_bwd_bf16", "t2v_frames_u8_to_nhwc8", "t2v_frames_u8_to_nhwc8_ragged", "t2v_scale_cast_f32_bf16", "t2v_cast_bf16_f32", "t2v_sqnorm_chunks", "t2v_adamw_prepare", "t2v_adamw_chunks", "t2v_adamw8bit_chunks", "t2v_adamw_ema_chunks", "t2v_adamw8bit_ema_chunks", "t2v_ema_swap_chunks", "t2v_counter_add", "t2v_upsample_nearest_fwd",
     "t2v_upsample_nearest_bwd", "t2v_copy_cols", "t2v_colsum", "t2v_colsum_f32", "t2v_softmax_fwd", "t2v_softmax_bwd",
     "t2v_timestep_embedding", "t2v_attn_small_fwd", "t2v_attn_small_bwd",
@@ -116,6 +122,7 @@ def _declare(lib):
     lib.t2v_nhwc8_to_latents.argtypes = [vp, vp] + [i32] * 4 + [vp]
     lib.t2v_mse_loss.argtypes = [vp] * 5 + [i32] * 4 + [vp]
     lib.t2v_velocity_mse_loss.argtypes = [vp] * 8 + [i32] * 4 + [vp]
+    lib.t2v_diffusion_loss.argtypes = [vp] * 5 + [ctypes.POINTER(LossParams)] + [vp] * 3 + [i32] * 4 + [vp]
     lib.t2v_vae_sample.argtypes = [vp, vp, vp, i32, i32, i32, f32, vp]
     lib.t2v_geglu_fwd.argtypes = [vp, vp, i64, i32, vp]
     lib.t2v_geglu_bwd.argtypes = [vp, vp, vp, i64, i32, vp]

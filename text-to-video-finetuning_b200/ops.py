@@ -922,3 +922,24 @@ class _VelocityMseLoss(Function):
 
 def velocity_mse_loss_nhwc8(pred, x0, noise, alphas_cumprod, timesteps):
     return _VelocityMseLoss.apply(pred, x0, noise, alphas_cumprod, timesteps)
+
+
+class _DiffusionLoss(Function):
+    """The Min-SNR-gamma weighted and / or pseudo-Huber objective of a step.LossObjective (snr_gamma, loss_type,
+    huber_schedule, huber_c), forward and backward in one kernel each: the noise target, or the velocity when x0 is given."""
+
+    @staticmethod
+    def forward(ctx, pred, x0, noise, alphas_cumprod, timesteps, objective):
+        ctx.objective = objective
+        ctx.save_for_backward(pred, x0, noise, alphas_cumprod, timesteps)
+        return prims.diffusion_loss_fwd(pred, x0, noise, alphas_cumprod, timesteps, objective)
+
+    @staticmethod
+    def backward(ctx, g):
+        pred, x0, noise, abar, t = ctx.saved_tensors
+        return prims.diffusion_loss_bwd(pred, x0, noise, abar, t, ctx.objective, _cont(g.float())), None, None, None, None, None
+
+
+def diffusion_loss_nhwc8(pred, x0, noise, alphas_cumprod, timesteps, objective):
+    """x0: the clean latents for a v-prediction model, None for epsilon."""
+    return _DiffusionLoss.apply(pred, x0, noise, alphas_cumprod, timesteps, objective)

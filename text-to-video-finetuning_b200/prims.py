@@ -717,3 +717,47 @@ def velocity_mse_loss_bwd(pred, x0, noise, alphas_cumprod, timesteps, gout):
     native.check(native.lib().t2v_velocity_mse_loss(_p(pred), _p(x0), _p(noise), _p(alphas_cumprod), _p(timesteps), _p(None), _p(gout),
                                                     _p(dpred), B, C, F, H * W, _stream()))
     return dpred
+
+
+_LOSS_FORMS = {"l2": 0, "huber": 1, "smooth_l1": 2}             # T2V_LOSS_*
+_HUBER_SCHEDULES = {"constant": 0, "exponential": 1, "snr": 2}   # T2V_HUBER_*
+
+
+def _loss_params(objective, x0, alphas_cumprod):
+    """native.LossParams of a step.LossObjective; x0 given selects the velocity target (T2V_PRED_V)."""
+    return native.LossParams(int(x0 is not None), _LOSS_FORMS[objective.loss_type], _HUBER_SCHEDULES[objective.huber_schedule],
+                             alphas_cumprod.numel(), float(objective.huber_c) if objective.loss_type != "l2" else 0.0,
+                             float(objective.snr_gamma or 0.0))
+
+
+def _chk_diffusion(pred, x0, noise, alphas_cumprod, timesteps):
+    _chk_bf16(pred)
+    _chk_f32(noise, alphas_cumprod)
+    if x0 is not None:
+        _chk_f32(x0)
+        assert x0.shape == noise.shape, (x0.shape, noise.shape)
+    assert timesteps.dtype == torch.int64 and timesteps.is_cuda and timesteps.is_contiguous(), timesteps.dtype
+    assert timesteps.shape == (noise.shape[0],), (timesteps.shape, noise.shape)
+
+
+def diffusion_loss_fwd(pred, x0, noise, alphas_cumprod, timesteps, objective):
+    """sum_e w_b psi(pred - y) / numel (t2v_diffusion_loss): `objective` a step.LossObjective (snr_gamma, loss_type,
+    huber_schedule, huber_c); y the noise, or the velocity when x0 is given.  pred [B*F,H,W,8] bf16, the rest fp32."""
+    _chk_diffusion(pred, x0, noise, alphas_cumprod, timesteps)
+    B, C, F, H, W = noise.shape
+    loss = torch.empty((), device=pred.device, dtype=torch.float32)
+    params = _loss_params(objective, x0, alphas_cumprod)
+    native.check(native.lib().t2v_diffusion_loss(_p(pred), _p(noise), _p(x0), _p(alphas_cumprod), _p(timesteps), ctypes.byref(params),
+                                                 _p(loss), _p(None), _p(None), B, C, F, H * W, _stream()))
+    return loss
+
+
+def diffusion_loss_bwd(pred, x0, noise, alphas_cumprod, timesteps, objective, gout):
+    """dpred = gout w_b psi'(pred - y) / numel, channels-last bf16 like pred."""
+    _chk_diffusion(pred, x0, noise, alphas_cumprod, timesteps)
+    B, C, F, H, W = noise.shape
+    dpred = torch.empty_like(pred)
+    params = _loss_params(objective, x0, alphas_cumprod)
+    native.check(native.lib().t2v_diffusion_loss(_p(pred), _p(noise), _p(x0), _p(alphas_cumprod), _p(timesteps), ctypes.byref(params),
+                                                 _p(None), _p(gout), _p(dpred), B, C, F, H * W, _stream()))
+    return dpred

@@ -5,6 +5,7 @@ the data-parallel step object used by train.py and bench.py."""
 import json
 import math
 import os
+from typing import NamedTuple, Optional
 
 import torch
 import torch.distributed as dist
@@ -14,6 +15,49 @@ from .runtime import GradientBuckets, GraphedStep, ParamArena, allreduce_gradien
 
 PREDICTION_TYPES = ("epsilon", "v_prediction")
 BETA_SCHEDULES = ("linear", "scaled_linear", "squaredcos_cap_v2")
+LOSS_TYPES = ("l2", "huber", "smooth_l1")
+HUBER_SCHEDULES = ("constant", "exponential", "snr")
+
+
+class LossObjective(NamedTuple):
+    """The per-pass training objective (diffusers' --snr_gamma, --loss_type, --huber_schedule, --huber_c), for B samples
+    with a_b = alphas_cumprod[t_b], d = pred - target:
+        loss = mean_b(w_b * mean_{c,f,h,w} psi(d))
+        psi  'l2': d^2   'huber': 2 c_b (sqrt(d^2 + c_b^2) - c_b)   'smooth_l1': 2 (sqrt(d^2 + c_b^2) - c_b)
+        c_b  'constant': huber_c   'exponential': huber_c ** (t_b / T)
+             'snr': (1 - huber_c) / (1 + sigma_b)^2 + huber_c, sigma_b = sqrt((1 - a_b) / a_b)   (huber_c at a_b = 0)
+        w_b  snr_gamma None: 1; else, with snr_b = a_b / (1 - a_b), min(snr_b, gamma) / snr_b for 'epsilon' (1 at a_b = 0)
+             and min(snr_b, gamma) / (snr_b + 1) for 'v_prediction' (0 at a_b = 0)   (Hang et al. 2023, Min-SNR-gamma)
+    Build it with loss_objective(), which validates the values."""
+    snr_gamma: Optional[float] = None
+    loss_type: str = "l2"
+    huber_schedule: str = "snr"
+    huber_c: float = 0.1
+
+    @property
+    def plain(self):
+        """The unweighted MSE: the step then runs mse_loss / velocity_mse_loss, the kernels of the default objective."""
+        return self.loss_type == "l2" and self.snr_gamma is None
+
+
+def loss_objective(snr_gamma=None, loss_type="l2", huber_schedule="snr", huber_c=0.1):
+    """A validated LossObjective.  An unknown loss_type or huber_schedule, snr_gamma <= 0, or (for 'huber' / 'smooth_l1')
+    huber_c <= 0 or, with 'exponential', huber_c > 1 raises ValueError.  Under 'l2' huber_c is not used."""
+    if loss_type not in LOSS_TYPES:
+        raise ValueError(f"loss_type {loss_type!r} is not supported; expected one of {LOSS_TYPES}")
+    if huber_schedule not in HUBER_SCHEDULES:
+        raise ValueError(f"huber_schedule {huber_schedule!r} is not supported; expected one of {HUBER_SCHEDULES}")
+    if snr_gamma is not None:
+        if isinstance(snr_gamma, bool) or not isinstance(snr_gamma, (int, float)) or not snr_gamma > 0:
+            raise ValueError(f"snr_gamma = {snr_gamma!r}: expected None or a number > 0")
+        snr_gamma = float(snr_gamma)
+    if loss_type != "l2":
+        if isinstance(huber_c, bool) or not isinstance(huber_c, (int, float)) or not (huber_c > 0 and math.isfinite(huber_c)):
+            raise ValueError(f"huber_c = {huber_c!r}: expected a finite number > 0")
+        if huber_schedule == "exponential" and huber_c > 1:
+            raise ValueError(f"huber_c = {huber_c!r}: the 'exponential' huber_schedule needs huber_c <= 1")
+        huber_c = float(huber_c)
+    return LossObjective(snr_gamma, loss_type, huber_schedule, huber_c)
 
 
 def ddpm_alphas_cumprod(num_train_timesteps=1000, beta_start=0.00085, beta_end=0.012, device=None):
@@ -83,19 +127,27 @@ def sample_noise(latents, noise_strength=0.0, use_offset_noise=False, generator=
     return noise
 
 
-def finetune_loss(unet, latents, noise, timesteps, encoder_hidden_states, alphas_cumprod, return_pred=False, prediction_type="epsilon"):
+def finetune_loss(unet, latents, noise, timesteps, encoder_hidden_states, alphas_cumprod, return_pred=False, prediction_type="epsilon",
+                  snr_gamma=None, loss_type="l2", huber_schedule="snr", huber_c=0.1):
     """One UNet pass of finetune_unet:
        noisy = add_noise(latents, noise, t)  ->  pred = unet(noisy, t, text)  ->  mse(pred.float(), target.float())
     with target = noise for prediction_type 'epsilon' and get_velocity(latents, noise, t) for 'v_prediction' (train.py:792-800).
     add_noise is fused into the layout-conversion kernel at the input, the loss reads the channels-last prediction
-    directly (and forms the velocity per element), so no (B,C,F,H,W) activation is ever materialised."""
+    directly (and forms the velocity per element), so no (B,C,F,H,W) activation is ever materialised.
+    snr_gamma / loss_type / huber_schedule / huber_c replace the MSE by the objective of LossObjective; with their defaults
+    the loss is the MSE above."""
     if prediction_type not in PREDICTION_TYPES:
         raise ValueError(f"prediction_type {prediction_type!r} is not supported; expected one of {PREDICTION_TYPES}")
+    objective = loss_objective(snr_gamma, loss_type, huber_schedule, huber_c)
     B, C, F, H, W = latents.shape
     x = prims.latents_to_nhwc8(latents.float().contiguous(), noise.float().contiguous(), alphas_cumprod, timesteps.to(torch.int64).contiguous())
     text = unet.prepare_text(encoder_hidden_states)
     pred = unet.forward_channels_last(x, timesteps.to(torch.int64).contiguous(), text, B, F)
-    if prediction_type == "v_prediction":
+    if not objective.plain:
+        x0 = latents.float().contiguous() if prediction_type == "v_prediction" else None
+        loss = ops.diffusion_loss_nhwc8(pred, x0, noise.float().contiguous(), alphas_cumprod, timesteps.to(torch.int64).contiguous(),
+                                        objective)
+    elif prediction_type == "v_prediction":
         loss = ops.velocity_mse_loss_nhwc8(pred, latents.float().contiguous(), noise.float().contiguous(), alphas_cumprod,
                                            timesteps.to(torch.int64).contiguous())
     else:
@@ -122,6 +174,8 @@ class DataParallelStep:
         buffer is zeroed at the start of each window and the shadow is re-cast from the masters every call.
 
     `prediction_type` picks the loss target of every pass: the noise ('epsilon') or the velocity ('v_prediction').
+    `snr_gamma`, `loss_type`, `huber_schedule` and `huber_c` pick the objective (LossObjective, validated by loss_objective);
+    each pass takes it, and the two passes' losses are summed and scaled by 1 / accumulation as the MSE's are.
 
     `text_encoder` (a text_encoder.CLIPTextModel that trains: cloneofsimo LoRA injected, `use_text_lora`, and/or parameters
     unfrozen by `train_text_encoder`): the call then takes the prompt token ids (B, L) in place of the text states, and the
@@ -134,9 +188,10 @@ class DataParallelStep:
     trainable projection weights are read through the arena's bf16 shadow."""
 
     def __init__(self, unet, alphas_cumprod, passes=1, use_graph=False, adopt=True, optimizer=None, accumulation=1,
-                 prediction_type="epsilon", text_encoder=None):
+                 prediction_type="epsilon", text_encoder=None, snr_gamma=None, loss_type="l2", huber_schedule="snr", huber_c=0.1):
         if prediction_type not in PREDICTION_TYPES:
             raise ValueError(f"prediction_type {prediction_type!r} is not supported; expected one of {PREDICTION_TYPES}")
+        self.objective = loss_objective(snr_gamma, loss_type, huber_schedule, huber_c)
         self.unet = unet
         self.abar = alphas_cumprod
         self.prediction_type = prediction_type
@@ -197,7 +252,8 @@ class DataParallelStep:
             else:
                 runs = [(latents, noise, states)]
         for i, (lat, nz, st) in enumerate(runs):
-            loss = finetune_loss(self.unet, lat, nz, timesteps, st, self.abar, prediction_type=self.prediction_type)
+            loss = finetune_loss(self.unet, lat, nz, timesteps, st, self.abar, prediction_type=self.prediction_type,
+                                 **self.objective._asdict())
             if overlap:
                 self.buckets.armed = i == len(runs) - 1   # gradients are final only in the last pass
             loss.backward(self._gscale if self.accumulation > 1 else None)

@@ -35,7 +35,7 @@ import torch.distributed as dist
 
 from .models.unet_3d_condition import UNet3DConditionModel
 from .ops import MAX_FRAMES
-from .step import DataParallelStep, load_noise_schedule, sample_noise
+from .step import DataParallelStep, load_noise_schedule, loss_objective, sample_noise
 from .utils.lora_handler import LORA_VERSIONS, LoraHandler
 
 already_printed_trainables = False
@@ -250,6 +250,10 @@ def main(
     lora_text_dropout: float = 0.1,
     logger_type: str = "tensorboard",
     save_training_state: bool = False,
+    snr_gamma: Optional[float] = None,
+    loss_type: str = "l2",
+    huber_schedule: str = "snr",
+    huber_c: float = 0.1,
     **kwargs,
 ):
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -279,6 +283,9 @@ def main(
     # noise schedule and loss target of the checkpoint (train.py:119, 792-800); an unsupported config fails here, before any
     # weights move.  `rescale_schedule` stays a no-op: in the reference it never reaches add_noise (SURVEY H5).
     abar, prediction_type = load_noise_schedule(pretrained_model_path)
+    # the objective (Min-SNR-gamma weighting, pseudo-Huber / smooth-L1 loss) is configuration, not training state: a resumed
+    # run takes it from this call, like the learning rate
+    objective = loss_objective(snr_gamma, loss_type, huber_schedule, huber_c)
     # temporal attention runs on clips of 1..256 frames (attn_small.cu); a longer clip fails here, not in the first step
     for section, key, data in (("train_data", "n_sample_frames", train_data), ("validation_data", "num_frames", validation_data)):
         frames = int((data or {}).get(key, 16))
@@ -341,7 +348,7 @@ def main(
     abar = abar.to(dev)
     use_graph = bool(kwargs.get("use_cuda_graph", dev.type == "cuda"))   # replay the whole step as one CUDA graph (static shapes)
     stepper = DataParallelStep(unet, abar, passes=2, use_graph=use_graph, accumulation=gradient_accumulation_steps,
-                               prediction_type=prediction_type, text_encoder=text_encoder)
+                               prediction_type=prediction_type, text_encoder=text_encoder, **objective._asdict())
     # parameters now live in the flat arena.  Every rank must start from rank 0's weights (DDP does this at wrap time).
     if world > 1:
         dist.broadcast(stepper.arena.master, src=0)
