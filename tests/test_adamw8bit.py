@@ -1,7 +1,7 @@
 """Blockwise 8-bit AdamW (optim.AdamW8bit, `use_8bit_adam`): the quantisation maps against a committed table, small tensors
 against torch.optim.AdamW, one step from zero state against the stated quantisation rule, convergence, `train.main`, the
-compact state size; on the GPU the CUDA kernel against its fp32 restatement (tests/adamw8bit_ref.py), checkpoint round trips
-and the CUDA-graph step."""
+compact state size; on the GPU checkpoint round trips and the CUDA-graph step (the kernel's element-wise check at every launch
+of the training steps is tests/test_optim_step_gpu.py)."""
 import json
 import os
 
@@ -201,7 +201,7 @@ def test_state_is_compact():
     assert want < 8 * sum(p.numel() for p in trainable) / 3
 
 
-# ---------------------------------------------------------------------------------------------------- GPU: kernel vs reference
+# ---------------------------------------------------------------------------------------------------- GPU: kernel cases (tests/test_ema_gpu.py)
 def _kernel_case(seed):
     """Four tensors in a flat arena: 8-bit with a ragged 64-element last block, 8-bit over two chunk rows with a ragged
     320-element last row, a 32-bit one and 8-bit with a ragged 128-element block that has no bf16 shadow.  Two
@@ -239,41 +239,6 @@ def _hp(step):
     for lr, b1, b2, eps, wd, scale in ((1e-3, 0.9, 0.999, 1e-8, 1e-2, 0.7), (5e-4, 0.8, 0.99, 1e-6, 0.0, 1.0)):
         out.append(torch.tensor([lr, b1, b2, eps, wd, 1 - b1 ** step, (1 - b2 ** step) ** 0.5, scale], dtype=torch.float32))
     return out
-
-
-@gpu
-@pytest.mark.parametrize("bf16_grad", [False, True])
-@pytest.mark.parametrize("zero_grad", [False, True])
-def test_kernel_matches_reference(bf16_grad, zero_grad):
-    from t2v_b200 import prims
-    from t2v_b200.optim import dynamic_map
-    st, tables, n_shadow, mask8, gen = _kernel_case(5)
-    qmaps = torch.cat([dynamic_map(True), dynamic_map(False)])
-    dev = {k: v.cuda() for k, v in st.items()}
-    for step in (1, 2, 3):
-        g = torch.randn(st["p"].numel(), generator=gen) * 0.1
-        g16 = (torch.randn(st["p"].numel(), generator=gen) * 0.1).bfloat16() if bf16_grad else None
-        host = {k: v.cpu().clone() for k, v in dev.items()}      # the reference starts from the kernel's state of this step
-        host["g"], dev["g"] = g.clone(), g.cuda()
-        for table, hp in zip(tables, _hp(step)):
-            ref.adamw8bit_chunks(host["p"], host["g"], host["shadow"], n_shadow, table, hp, qmaps, host["m32"], host["v32"], host["code_m"],
-                                 host["code_v"], host["absmax_m"], host["absmax_v"], zero_grad, g16)
-            prims.adamw8bit_chunks(dev["p"], dev["g"], dev["shadow"], n_shadow, table.cuda(), hp.cuda(), qmaps.cuda(), dev["m32"], dev["v32"],
-                                   dev["code_m"], dev["code_v"], dev["absmax_m"], dev["absmax_v"], zero_grad,
-                                   None if g16 is None else g16.cuda())
-        torch.cuda.synchronize()
-        out = {k: v.cpu() for k, v in dev.items()}
-        for k in ("code_m", "code_v"):
-            a, b = out[k][mask8].long(), host[k][mask8].long()
-            assert int((a - b).abs().max()) <= 1, (step, k)
-            assert float((a == b).float().mean()) >= 0.9999, (step, k, float((a == b).float().mean()))
-        for k in ("absmax_m", "absmax_v"):
-            assert bool(((out[k] - host[k]).abs() <= 1e-6 * host[k].abs()).all()), (step, k)
-        for k in ("p", "m32", "v32"):
-            assert torch.allclose(out[k], host[k], rtol=1e-5, atol=1e-7), (step, k, float((out[k] - host[k]).abs().max()))
-        assert torch.equal(out["shadow"][:n_shadow], out["p"][:n_shadow].bfloat16())
-        assert torch.equal(out["shadow"][n_shadow:], st["shadow"][n_shadow:])
-        assert torch.equal(out["g"], torch.zeros_like(g) if zero_grad else g)
 
 
 # ---------------------------------------------------------------------------------------------------- GPU: checkpoint, train.main

@@ -1,8 +1,9 @@
 """Every prims function a census workload calls is checked element by element somewhere: it is claimed by exactly one launch
-census (GEMM, attention, norm, glue; each has a float64 check of every recorded launch) or by ALLOWLIST, which names the test
+census (GEMM, attention, norm, glue, optimizer; each has a float64 check of every recorded launch) or by ALLOWLIST, which names the test
 that covers it and why it sits outside a census.  A new kernel that the training steps launch without a check fails here.
-The workloads are those of tests/golden/make_glue_launches.py (a superset of the other censuses' workloads), run once on the meta
-device with every public prims function wrapped by a recorder."""
+The workloads are those of tests/golden/make_glue_launches.py (a superset of the other kernel censuses' workloads) and of
+tests/golden/make_optim_launches.py (the optimizer steps, the stable-LoRA pass and the gradient compression), run once on the
+meta device with every public prims function wrapped by a recorder."""
 import os
 import sys
 
@@ -14,24 +15,16 @@ sys.path.insert(0, os.path.join(HERE, "golden"))
 import make_attn_launches as MA   # noqa: E402
 import make_glue_launches as MG   # noqa: E402
 import make_norm_launches as MN   # noqa: E402
+import make_optim_launches as MO   # noqa: E402
 
 CENSUSES = {
     "gemm": ("conv_fwd", "conv_dgrad", "conv_wgrad", "bgemm"),                       # tests/test_gemm_step_gpu.py
     "attention": tuple(k for k in MA.KINDS if k != "composite") + ("softmax_fwd", "softmax_bwd"),   # tests/test_attn_step_gpu.py
     "norm": MN.KINDS,                                                                  # tests/test_norm_step_gpu.py
     "glue": MG.KINDS,                                                                  # tests/test_glue_step_gpu.py
+    "optimizer": MO.KINDS,                                                             # tests/test_optim_step_gpu.py
 }
 ALLOWLIST = {
-    "sqnorm_chunks": "optimizer (after the backward pass): tests/test_fused_adamw.py through optim.FusedAdamW",
-    "adamw_prepare": "optimizer: tests/test_fused_adamw.py through optim.FusedAdamW",
-    "adamw_chunks": "optimizer: tests/test_fused_adamw.py through optim.FusedAdamW",
-    "adamw8bit_chunks": "optimizer: tests/test_adamw8bit.py",
-    "adamw_ema_chunks": "optimizer: tests/test_ema_gpu.py",
-    "adamw8bit_ema_chunks": "optimizer: tests/test_ema_gpu.py",
-    "ema_swap_chunks": "optimizer: tests/test_ema_gpu.py",
-    "lora_delta_merge": "stable_lora only: tests/test_stable_lora_gpu.py",
-    "lora_delta_grad": "stable_lora only: tests/test_stable_lora_gpu.py",
-    "scale_cast_f32_bf16": "data-parallel only (gradient compression before the all-reduce): tests/test_data_parallel_cpu.py, compress=True",
     "out_hw": "host helper: no kernel",
     "stats_alloc": "host helper: a zeroed buffer, no kernel",
 }
@@ -63,6 +56,7 @@ def called():
             return run
 
         MG.run_workloads(observe=observe)
+        MO.run_workloads(observe=observe)
         _CALLED.append(sorted(seen))
     return _CALLED[0]
 

@@ -159,11 +159,15 @@ class FusedAdamW(torch.optim.Optimizer):
             chunks = self._table(params)
             if not chunks:
                 continue
-            table = torch.tensor(chunks, dtype=torch.int64, device=dev).contiguous()
+            # each table is built on the host and kept there next to its device copy (the host copy is what a table built
+            # on the meta device can still be read from)
+            host = torch.tensor(chunks, dtype=torch.int64)
+            table = host.to(dev)
             sets.append({"groups": gis, "key": key, "chunks": table, "norm_chunks": table[:, :2].contiguous() if table.shape[1] > 2 else table,
-                         "n": sum(c[1] for c in chunks)})
+                         "n": sum(c[1] for c in chunks), "chunks_host": host})
             if self.ema is not None:
-                sets[-1]["ema_chunks"] = torch.tensor(self._ema_rows(chunks), dtype=torch.int64, device=dev)
+                ema_host = torch.tensor(self._ema_rows(chunks), dtype=torch.int64)
+                sets[-1]["ema_chunks"], sets[-1]["ema_chunks_host"] = ema_host.to(dev), ema_host
         if not sets:
             raise ValueError("FusedAdamW: no trainable parameters")
         if self.ema is not None:   # (arena offset, length, EMA offset) over every set: the rows ema_weights() swaps
@@ -316,8 +320,9 @@ class AdamW8bit(FusedAdamW):
             else:
                 self._layout[id(p)] = (32, n32)
                 n32 += n
-        self.qmaps = torch.cat([dynamic_map(True), dynamic_map(False)]).to(dev)
-        zero_m = int((self.qmaps[:256] == 0).nonzero()[0, 0])
+        qmaps = torch.cat([dynamic_map(True), dynamic_map(False)])
+        zero_m = int((qmaps[:256] == 0).nonzero()[0, 0])   # on the host map: a meta-device map has no values
+        self.qmaps = qmaps.to(dev)
         self.code_m = torch.full((n8,), zero_m, device=dev, dtype=torch.uint8)
         self.code_v = torch.zeros(n8, device=dev, dtype=torch.uint8)   # the unsigned map starts at 0.0
         self.absmax_m = torch.zeros(n8 // QBLOCK, device=dev, dtype=torch.float32)
